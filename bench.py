@@ -368,6 +368,26 @@ def real_stream_b200(eng, repeats=3, copies=4):
     return out
 
 
+DUMP_LUMA_SAMPLES, DUMP_CHROMA_SAMPLES = 1 << 18, 1 << 16
+
+
+def dump_outputs(out_dir, eng, step_pics):
+    """Writes the pictures of the last timed step that are still held by their DPB slots (a later picture of the same step may
+    reuse a slot), in decode order: a fixed seeded sample of every plane (luma.npy, cb.npy, cr.npy: float32, one row per
+    picture), every plane's sample sum (plane_sums.npy: float64, pictures x 3) and the pictures' POCs (poc.npy: float64).
+    About 1.5 MB per 4K picture, under 64 MB for the 28 pictures a step leaves."""
+    last = {p.params.dst_slot: i for i, p in enumerate(step_pics)}
+    pics = [step_pics[i] for i in sorted(last.values())]
+    rng = np.random.default_rng(20240601)
+    planes = [eng.read_slot(p.params.dst_slot, p.params) for p in pics]
+    idx = [rng.choice(pl.size, min(pl.size, n), replace=False) for pl, n in zip(planes[0], (DUMP_LUMA_SAMPLES, DUMP_CHROMA_SAMPLES, DUMP_CHROMA_SAMPLES))]
+    os.makedirs(out_dir, exist_ok=True)
+    for c, name in enumerate(("luma", "cb", "cr")):
+        np.save(os.path.join(out_dir, name + ".npy"), np.stack([pl[c].reshape(-1)[idx[c]] for pl in planes]).astype(np.float32))
+    np.save(os.path.join(out_dir, "plane_sums.npy"), np.array([[pl[c].sum(dtype=np.float64) for c in range(3)] for pl in planes]))
+    np.save(os.path.join(out_dir, "poc.npy"), np.array([p.params.poc for p in pics], np.float64))
+
+
 def run_config(name, eng, torch, dist, stream, a, rank, local_rank, world, headline):
     """Runs one bench configuration on this rank's engine: `value` (records resident in HBM, pictures pipelined over the engine's
     streams), the per-stage one-stream pass behind `roofline`, and `e2e` (host records in, pictures out).  Returns the
@@ -440,6 +460,9 @@ def run_config(name, eng, torch, dist, stream, a, rank, local_rank, world, headl
     ms_res = timed(step_resident, steps)
     launches = eng.launch_count() - l0
     clk = clocks.stop()
+    if headline and a.dump_outputs and rank == 0:
+        v = (counter["step"] - 1) % STEP_VARIANTS
+        dump_outputs(a.dump_outputs, eng, seq[32 * v:32 * (v + 1)])
     # ---- per-stage kernel times: CUDA events around every stage of every picture on the launching stream.  Stages of
     #      different pictures must not overlap for that, so this pass runs the same steps on ONE stream ----
     eng.enable_timing(True)
@@ -471,8 +494,8 @@ def run_config(name, eng, torch, dist, stream, a, rank, local_rank, world, headl
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except OSError:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6.65 TB/s (B200_PROFILING.md)"
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "data sheet 3.35 TB/s (H100 SXM HBM3)"
     alg = algorithmic_bytes(seq[:32], bd)
     n_inter = sum(1 for p in seq[:32] if len(p.pus))
     per_stage = {}
@@ -482,18 +505,13 @@ def run_config(name, eng, torch, dist, stream, a, rank, local_rank, world, headl
         per_stage[k] = {"ms_per_step": round(ms, 4), "algorithmic_MB_per_step": round(alg[k] / 1e6, 2), "achieved_gbs": round(gbs, 1),
                         "frac": round(gbs / peak, 4)}
     dominant = max(per_stage, key=lambda k: per_stage[k]["ms_per_step"])
-    traffic = {}
-    try:  # dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu --set full capture
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "dram_traffic_per_launch.json")))
-    except (OSError, ValueError):
-        pass
     mc_kernel = "k_inter_pred_tma" if bd == 8 and not os.environ.get("B200_MC_LEGACY") else ("k_inter_pred8" if bd == 8 else "k_inter_pred<u16>")
 
     def roof(k):
         launches_per_step = max(1, {"inter_pred": n_inter, "recon": 32, "deblock": 64, "sao": 32}[k])
         return {"kernel": {"inter_pred": mc_kernel, "recon": "k_residual+k_intra", "deblock": "k_deblock<V>+<H>", "sao": "k_sao8" if bd == 8 else "k_sao_prep+k_sao<u16>"}[k],
                 "bound": "hbm", "achieved": per_stage[k]["achieved_gbs"], "peak": peak, "unit": "GB/s", "frac": per_stage[k]["frac"],
-                "traffic": traffic.get(k) if name == "main_ra_4k" else None, "peak_source": peak_src,
+                "peak_source": peak_src,
                 "avg_launch_ms": round(per_stage[k]["ms_per_step"] / launches_per_step, 5),
                 "algorithmic_bytes_per_launch": int(alg[k] / launches_per_step),
                 "timing": "CUDA events per stage on the launching stream, one-stream pass of %d steps right after the timed region" % stage_steps}
@@ -504,7 +522,7 @@ def run_config(name, eng, torch, dist, stream, a, rank, local_rank, world, headl
                       f"{width}x{height} {bd}-bit 4:2:0 synthetic command records ({cfg['kind']} structure of {name})",
                       "name": name, "pictures_per_step": 32,
                       "l2_policy": f"per-step working set ({len({p.params.dst_slot for p in seq})} DPB surfaces x {pic_bytes / 1e6:.1f} MB + {STEP_VARIANTS} x 32 record sets) "
-                                   "exceeds the 126 MB L2"},
+                                   "exceeds the 50 MB L2 of an H100"},
            "e2e": {"value": round(fps_e2e, 2), "unit": "frames/s", "h2d_bytes_per_step": h2d_bytes, "d2h_bytes_per_step": 32 * pic_bytes,
                    "inputs": "record arrays page-locked (cudaHostRegister), uploaded directly" if pinned else "pageable record arrays through pinned staging",
                    "ms_per_step": round(ms_e2e / steps, 4)},
@@ -529,6 +547,8 @@ def main():
     ap.add_argument("--height", type=int, default=H)
     ap.add_argument("--bit-depth", type=int, default=BD)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps of the headline config, write a seeded sample of the pictures its last step decoded to DIR/*.npy")
     a = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))

@@ -1,5 +1,5 @@
 /*
- * b200hevc.h — C ABI of the B200-native HEVC reconstruction engine.
+ * b200hevc.h — C ABI of the HEVC reconstruction engine for the H100 (sm_90a).
  *
  * This is the drop-in boundary for the per-CTB reconstruction hot path of
  * strukturag/libde265 (dequant + inverse DCT/DST + add-residual, luma/chroma MC

@@ -1,4 +1,4 @@
-"""In-tree build of the CUDA library (sm_100a only).  Used by __graft_entry__.build()."""
+"""In-tree build of the CUDA library (sm_90a, H100, only).  Used by __graft_entry__.build()."""
 import os
 import subprocess
 
@@ -7,7 +7,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libb200hevc.so")
 SOURCES = ["engine.cu", "recorder.cc"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC,-fvisibility=hidden",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC,-fvisibility=hidden",
               "-shared", "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
 
 

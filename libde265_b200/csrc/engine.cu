@@ -206,7 +206,7 @@ __global__ void k_extend_borders(uint8_t* p0, uint8_t* p1, uint8_t* p2, int pitc
 
 static void launch_extend_borders(const Surface& s, cudaStream_t st)
 {
-  dim3 grid(148 * 2, s.chroma ? 3 : 1);
+  dim3 grid(132 * 2, s.chroma ? 3 : 1);  // two CTAs per SM of an H100 SXM
   if (bytes_per_sample(s.bd_y) == 2)
     k_extend_borders<uint16_t><<<grid, 256, 0, st>>>(s.plane[0], s.plane[1], s.plane[2], s.pitch[0], s.pitch[1], s.w, s.h, s.cw, s.ch);
   else
@@ -363,12 +363,10 @@ struct b200_engine {
     if (use_helper) helper->wait(&helper_group);
     else pool.wait();
   }
-  int num_sms = 148;
+  int num_sms = 132;
   long long slot_depth[B200_MAX_SLOTS] = {}, tail_depth[B200_MAX_CTX] = {}, key_depth = 0;  // pick_ctx: dependency depths
   // one intra task per plane and region in every picture (default).  B200_INTRA_SPLIT=0: pictures with inter prediction merge the
-  // planes of a region into one task — fewer tasks, but each runs its segments in sequence (three dependent L2 round trips);
-  // measured with tickets in level order and 3 CTAs per SM: 4K B picture k_intra 0.25 ms split vs 0.28 ms merged, bench 3382 vs 3210
-  // frames/s
+  // planes of a region into one task — fewer tasks, but each runs its segments in sequence (three dependent L2 round trips)
   bool intra_split_planes = true;
   bool sched_rr = false;        // B200_SCHED=rr: plain round-robin placement (A/B measurements)
   int n_ind = 2, next_ind = 0, ind_run = 0;  // streams for pictures that read no reference (intra pictures), used round-robin (B200_IND_STREAMS)

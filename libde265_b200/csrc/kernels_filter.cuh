@@ -331,7 +331,7 @@ __global__ void __launch_bounds__(128) k_sao(DevPic pic, FilterArgs a)
 // -------------------------------------------------------------------------------------------------
 // k_sao8: SAO for 8-bit samples with byte-parallel arithmetic (CTB sizes 32 and 64; other cases run k_sao).
 // k_sao spends ~70 instructions per sample (one sample per step of an unrolled loop: classification, table look-up, clip) and is
-// bound by instruction issue at 39 us per 4K picture, 10x the time its 25 MB of traffic need.  Here a lane owns 16 samples x
+// bound by instruction issue, not by its 25 MB of traffic per 4K picture.  Here a lane owns 16 samples x
 // SAO8_R rows as 32-bit words and classifies / offsets four samples per instruction:
 //   * unsigned byte compare  x < y  =  bit 7 of  (~x & y) | (~(x ^ y) & ~((x | 0x80..) - (y & 0x7f..)))  (no carries between
 //     bytes), widened to a byte mask by one PRMT with sign replication;

@@ -34,7 +34,7 @@
 #define MCT_HD __host__ __device__ __forceinline__
 
 #ifndef MCT_THREADS
-#define MCT_THREADS 192                  // compute threads per CTA (warps 0..MCT_THREADS/32-1); one more warp is the producer. 576 pass-1 and 192 pass-2 tasks per big batch: 3 + 1 full rounds (128: 57.6 us, 192: 54.5 us, 256: 55.2 us per 4K B picture)
+#define MCT_THREADS 192                  // compute threads per CTA (warps 0..MCT_THREADS/32-1); one more warp is the producer. 576 pass-1 and 192 pass-2 tasks per big batch: 3 + 1 full rounds
 #endif
 #ifndef MCT_TLS
 #define MCT_TLS 32                       // tile-list items per batch with the small boxes (a power of two); half as many with the big ones
@@ -136,8 +136,7 @@ MCT_HD MctGeom mct_geom(int cls)
 
 #ifndef MCT_DB
 #define MCT_DB 1  // window buffers: 2 = the producer fetches a whole batch ahead (the boxes of batch n+1 land while batch n is computed).
-                  // Measured (4K B picture): 1 buffer x 3 CTAs/SM 57.9 us; 2 buffers x 2 CTAs/SM 61.5-62.2 us; 2 buffers of 16 items x
-                  // 3 CTAs/SM 61.3 us — the second buffer costs a resident CTA and buys nothing: 1 stays the default
+                  // The second buffer costs shared memory and with it resident CTAs per SM: 1 is the default.
 #endif
 struct MctShared {
   alignas(128) uint8_t win[MCT_DB][MCT_WIN_BYTES];

@@ -442,7 +442,7 @@ __device__ void tu_intra_large(const b200_tu& tu, const P* gsrc, int gstride, P*
   // ---- gather + substitution (intrapred.h:529-674); scan index s: 0 -> border[-2nT], 2nT -> border[0], 4nT -> border[2nT]
   // All (up to 129) neighbour samples are requested FIRST — up to five independent loads per lane, one L2 round trip — and the
   // availability scan / substitution then runs on registers.  (The loads used to sit inside the two chunk loops, each chunk's
-  // ballot waiting for its load: ten dependent round trips per large TU, ~8 us of the task's dependent latency.)
+  // ballot waiting for its load: ten dependent round trips per large TU.)
   {
     constexpr int MAXC = 5;  // ceil((4 * 32 + 1) / 32)
     int v[MAXC];
@@ -774,7 +774,7 @@ __global__ void __launch_bounds__(RC_THREADS, 3) k_intra(DevPic pic, ReconArgs a
           // Bounded: in a well-formed picture every dependency belongs to an earlier task, so the wait ends.  A record whose avail
           // bits name a unit of a later task (or its own) would spin forever: give up after spin_limit_ns (and at once when another
           // task already gave up), flag the picture and go on with whatever the neighbours hold.  The host reports
-          // B200_ERR_INVALID at the next synchronisation point.  Checked every 64th poll (~60 us): nothing on the polling path.
+          // B200_ERR_INVALID at the next synchronisation point.  Checked every 64th poll: nothing on the polling path.
           unsigned long long now;
           asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
           if (!t_wait0) t_wait0 = now;

@@ -25,7 +25,7 @@ def build_emulator():
     if os.path.exists(SO) and all(os.path.getmtime(SO) >= os.path.getmtime(d) for d in deps):
         return
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    subprocess.check_call([nvcc, "-O2", "-std=c++17", "-Xcompiler", "-fPIC,-fvisibility=hidden", "-shared", "-gencode", "arch=compute_100a,code=sm_100a",
+    subprocess.check_call([nvcc, "-O2", "-std=c++17", "-Xcompiler", "-fPIC,-fvisibility=hidden", "-shared", "-gencode", "arch=compute_90a,code=sm_90a",
                            "-I" + os.path.join(ROOT, "include"), "-I" + CSRC, "-o", SO, SRC])
 
 

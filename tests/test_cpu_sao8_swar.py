@@ -19,7 +19,7 @@ HDR = os.path.join(ROOT, "libde265_b200", "csrc", "sao8_swar.cuh")
 def lib():
     if not (os.path.exists(SO) and all(os.path.getmtime(SO) >= os.path.getmtime(d) for d in (SRC, HDR))):
         nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-        subprocess.check_call([nvcc, "-O2", "-std=c++17", "-Xcompiler", "-fPIC,-fvisibility=hidden", "-shared", "-gencode", "arch=compute_100a,code=sm_100a",
+        subprocess.check_call([nvcc, "-O2", "-std=c++17", "-Xcompiler", "-fPIC,-fvisibility=hidden", "-shared", "-gencode", "arch=compute_90a,code=sm_90a",
                                "-I" + os.path.dirname(HDR), "-o", SO, SRC])
     l = C.CDLL(SO)
     for f in ("sao8_check_lt", "sao8_check_apply", "sao8_check_eq_mask"):

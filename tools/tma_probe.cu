@@ -2,7 +2,7 @@
 // (reference windows of one MC unit: 23 rows of 32..80 bytes) can one SM fetch per microsecond from an L2/HBM-resident
 // padded 4K surface, against the same windows fetched with per-lane 16-byte loads + shared-memory stores?
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tma_probe tools/tma_probe.cu && ./tma_probe
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tma_probe tools/tma_probe.cu && ./tma_probe
 #include <cuda.h>
 #include <cuda_runtime.h>
 

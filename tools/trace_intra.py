@@ -37,7 +37,7 @@ for c in range(3):
     for k in sorted(set(cnt[plane == c])):
         m = (plane == c) & (cnt == k)
         print(f" plane {c} TUs/task {k:2d}: n={m.sum():6d} work mean {work[m].mean()/clk:7.2f} us  (log2 of first TU: {np.bincount(lg[m]).tolist()})")
-print("sum of work / 1e3:", work.sum() / clk / 1e3, "ms  => with", 148 * 3 * 8, "warps:", work.sum() / clk / 1e3 / (148 * 3 * 8), "ms")
+print("sum of work / 1e3:", work.sum() / clk / 1e3, "ms  => with", 132 * 3 * 8, "warps:", work.sum() / clk / 1e3 / (132 * 3 * 8), "ms")
 # ticket-order view (tickets are in DAG-level order): when are the tasks of each slice of the ticket range claimed / finished?
 idx = np.arange(n)
 base = t0.min()
