@@ -46,6 +46,9 @@ def _zorder(x, y):
 
 _Z = np.array([[_zorder(x, y) for x in range(16)] for y in range(16)], dtype=np.int64)  # [y4][x4] inside a 64x64 CTB
 
+# Reference border of a slot (B200_PAD_X / _Y / _CX / _CY of csrc/dev_common.cuh): MC windows further out are moved to this rim.
+_PAD_X, _PAD_Y, _PAD_CX, _PAD_CY = 128, 80, 64, 40
+
 
 class SynthPicture:
     """Holds the numpy arrays of one picture and a ctypes ``capi.Picture`` view of them."""
@@ -89,38 +92,68 @@ class SynthPicture:
 def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, ref_slots=(), log2_ctb=6, intra_frac=None,
                  weighted=False, deblock=True, sao=True, special_frac=0.01, cbf_prob=0.6, n_slices=1, scaling_list=False,
                  size_area=(0.10, 0.25, 0.35, 0.30), qp_range=(22, 37), far_mv_frac=0.01, tiles=(1, 1), lf_across_tiles=True,
-                 rdpcm_frac=0.0, rotate_frac=0.0, tskip_max_log2=2):
+                 rdpcm_frac=0.0, rotate_frac=0.0, tskip_max_log2=2, chroma_format_idc=1, bit_depth_chroma=None, chroma_qp_offsets=None,
+                 lf_offsets=None, weight_range="narrow", sao_offset="random", extreme_mv_frac=0.0, strong_smoothing=True,
+                 intra_smoothing_off=False, no_bfilter_on_bypass=False, pcm_lf_disable=False, slice_deblock_off_frac=0.0,
+                 slice_sao_off_frac=0.0, skip_sao=False):
     """Generate one picture.  ``size_area`` = fraction of the picture area coded as 64/32/16/8 CUs.
     ``tiles`` = (columns, rows) of uniformly spaced tiles (pps.cc uniform_spacing rule): CTBs are then coded in tile-scan
     order and intra availability stops at tile borders (intrapred.h:488-503); ``lf_across_tiles`` False also removes the
     deblocking edges on tile borders (deblock.cc:185-230) and lets SAO treat the neighbour tile as unavailable (sao.cc:157).
     ``rdpcm_frac`` / ``rotate_frac``: share of the transform-skip / bypass TUs that use RDPCM (RExt implicit/explicit rdpcm,
     transform.cc:425-432,566-578) resp. coefficient rotation (4x4 TUs of intra CUs, transform.cc:402-404);
-    ``tskip_max_log2``: largest transform-skip TU (RExt log2_max_transform_skip_block_size)."""
+    ``tskip_max_log2``: largest transform-skip TU (RExt log2_max_transform_skip_block_size).
+
+    Range knobs (each, at its default, draws no random number and changes nothing):
+    ``chroma_format_idc`` 0 (4:0:0: no chroma TUs, luma-only PCM) or 1; ``bit_depth_chroma`` (default: ``bit_depth``) for the
+    chroma PCM samples, QpBdOffsetC, log2wd_chroma, the chroma weight offsets and the SAO chroma offsets; ``qp_range`` may
+    start at -QpBdOffsetY; ``chroma_qp_offsets`` = (pps_cb, pps_cr); ``lf_offsets`` = (beta, tc) of every slice (the
+    slice_*_offset_div2 values times 2); ``weight_range`` "spec": weights (1 << denom) + [-128, 127] and offsets
+    [-128, 127] << (bd - 8) per plane, with the extremes -128 (one past the syntax's floor) and 255 always present;
+    ``sao_offset`` "max": every SAO offset at +-((1 << (min(bd, 10) - 5)) - 1) << log2_sao_offset_scale, scale drawn in
+    [0, bd - 10]; ``extreme_mv_frac``: share of the PUs touching the picture border whose MV components are -32768 / 32767 or
+    land just inside / outside the rim of the slot's reference border (any phase); ``strong_smoothing`` /
+    ``intra_smoothing_off``: the SPS flags; ``no_bfilter_on_bypass``: implicit RDPCM enabled (TU_NO_BOUNDARY_FILTER on the
+    intra TUs of bypass CUs, implicit RDPCM on their horizontal / vertical bypass and transform-skip TUs, as
+    integration/libde265_hooks.cc records them); ``pcm_lf_disable``: pcm_loop_filter_disable (PCM CUs in ``nofilt_map``);
+    ``slice_deblock_off_frac`` / ``slice_sao_off_frac``: share of the slices with deblocking off (their edges get bS 0) resp.
+    each SAO plane flag off; ``skip_sao``: PIC_SKIP_SAO."""
     assert width % 8 == 0 and height % 8 == 0
+    assert chroma_format_idc in (0, 1)
     rng = np.random.default_rng(seed)
     S = 1 << log2_ctb
     wctb, hctb = (width + S - 1) // S, (height + S - 1) // S
     w4, h4, w8, h8 = (width + 3) // 4, (height + 3) // 4, (width + 7) // 8, (height + 7) // 8
-    bdoff = 6 * (bit_depth - 8)
+    bd_c = bit_depth if bit_depth_chroma is None else bit_depth_chroma
+    bdoff, bdoff_c = 6 * (bit_depth - 8), 6 * (bd_c - 8)
     if intra_frac is None:
         intra_frac = 1.0 if pic_type == "I" else 0.08
     if pic_type != "I" and not ref_slots:
         raise ValueError("P/B pictures need ref_slots")
+    if qp_range[0] < -bdoff or qp_range[1] > 51:
+        raise ValueError(f"qp_range {qp_range}: QpY lies in [-{bdoff}, 51] at {bit_depth} bit")
     cb_off, cr_off = int(rng.integers(-3, 4)), int(rng.integers(-3, 4))
+    if chroma_qp_offsets is not None:
+        cb_off, cr_off = chroma_qp_offsets
 
     params = capi.PicParams()
     params.width, params.height = width, height
-    params.chroma_format_idc = 1
-    params.bit_depth_luma = params.bit_depth_chroma = bit_depth
+    params.chroma_format_idc = chroma_format_idc
+    params.bit_depth_luma, params.bit_depth_chroma = bit_depth, bd_c
     params.log2_ctb_size = log2_ctb
-    flags = capi.PIC_STRONG_INTRA_SMOOTHING | (capi.PIC_LF_ACROSS_TILES if lf_across_tiles else 0)
+    flags = (capi.PIC_STRONG_INTRA_SMOOTHING if strong_smoothing else 0) | (capi.PIC_LF_ACROSS_TILES if lf_across_tiles else 0)
     if sao:
         flags |= capi.PIC_SAO_ENABLED
     if not deblock:
         flags |= capi.PIC_SKIP_DEBLOCK
     if scaling_list:
         flags |= capi.PIC_SCALING_LIST
+    if intra_smoothing_off:
+        flags |= capi.PIC_INTRA_SMOOTHING_OFF
+    if pcm_lf_disable:
+        flags |= capi.PIC_PCM_LF_DISABLE
+    if skip_sao:
+        flags |= capi.PIC_SKIP_SAO
     params.flags = flags
     params.pps_cb_qp_offset, params.pps_cr_qp_offset = cb_off, cr_off
     params.dst_slot = dst_slot
@@ -151,9 +184,18 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
         slices[i]["slice_addr_rs"] = ctb_order[bounds[i]]
         slices[i]["beta_offset"] = 2 * int(rng.integers(-3, 4))
         slices[i]["tc_offset"] = 2 * int(rng.integers(-3, 4))
+        if lf_offsets is not None:
+            slices[i]["beta_offset"], slices[i]["tc_offset"] = lf_offsets
         f = capi.SLICE_SAO_LUMA | capi.SLICE_SAO_CHROMA
         if n_slices == 1 or rng.random() < 0.5:
             f |= capi.SLICE_LF_ACROSS_SLICES
+        if slice_deblock_off_frac and rng.random() < slice_deblock_off_frac:
+            f |= capi.SLICE_DEBLOCK_DISABLED
+        if slice_sao_off_frac:
+            if rng.random() < slice_sao_off_frac:
+                f &= ~capi.SLICE_SAO_LUMA
+            if rng.random() < slice_sao_off_frac:
+                f &= ~capi.SLICE_SAO_CHROMA
         slices[i]["flags"] = f
         ctb_slice[np.array(ctb_order[bounds[i]:bounds[i + 1]])] = i
 
@@ -162,12 +204,25 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
     if weighted and pic_type != "I":
         nw = 4
         weights = np.zeros(nw, WT_DT)
-        shift1 = max(2, 14 - bit_depth)
+        shift1, shift1_c = max(2, 14 - bit_depth), max(2, 14 - bd_c)
+        o_scale = np.array([1 << (bit_depth - 8), 1 << (bd_c - 8), 1 << (bd_c - 8)])  # per plane: luma, Cb, Cr
         for i in range(nw):
-            weights[i]["w"] = rng.integers(-40, 120, size=(2, 3))
-            weights[i]["o"] = rng.integers(-20, 21, size=(2, 3)) * (1 << (bit_depth - 8))
-            weights[i]["log2wd_luma"] = int(rng.integers(0, 8)) + shift1
-            weights[i]["log2wd_chroma"] = int(rng.integers(0, 8)) + shift1
+            if weight_range == "spec":  # pred_weight_table: delta weights and offsets in [-128, 127] (offsets in 8-bit units)
+                dl, dc = int(rng.integers(0, 8)), int(rng.integers(0, 8))
+                weights[i]["w"] = rng.integers(-128, 128, size=(2, 3)) + np.array([1 << dl, 1 << dc, 1 << dc])
+                weights[i]["o"] = rng.integers(-128, 128, size=(2, 3)) * o_scale
+            else:
+                assert weight_range == "narrow"
+                weights[i]["w"] = rng.integers(-40, 120, size=(2, 3))
+                weights[i]["o"] = rng.integers(-20, 21, size=(2, 3)) * o_scale
+                dl, dc = int(rng.integers(0, 8)), int(rng.integers(0, 8))
+            weights[i]["log2wd_luma"] = dl + shift1
+            weights[i]["log2wd_chroma"] = dc + shift1_c
+        if weight_range == "spec":  # the extremes on every plane and list: entry 0 lowest, entry 1 highest, entries 2/3 mixed
+            weights[0]["w"], weights[0]["o"] = -128, -128 * o_scale
+            weights[1]["w"], weights[1]["o"] = 255, 127 * o_scale
+            weights[2]["w"][0], weights[2]["w"][1] = [255, -128, 255], [-128, 255, -128]
+            weights[3]["o"][0], weights[3]["o"][1] = [127, -128, 127] * o_scale, [-128, 127, -128] * o_scale
 
     scaling = None
     if scaling_list:
@@ -251,9 +306,9 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
             n_coeff_total[0] += n
 
     def qp_primes(qpy):
-        qpi_cb = min(max(qpy + cb_off, -bdoff), 57)
-        qpi_cr = min(max(qpy + cr_off, -bdoff), 57)
-        return qpy + bdoff, max(0, _table8_22(qpi_cb) + bdoff), max(0, _table8_22(qpi_cr) + bdoff)
+        qpi_cb = min(max(qpy + cb_off, -bdoff_c), 57)
+        qpi_cr = min(max(qpy + cr_off, -bdoff_c), 57)
+        return qpy + bdoff, max(0, _table8_22(qpi_cb) + bdoff_c), max(0, _table8_22(qpi_cr) + bdoff_c)
 
     def tu_block(x, y, log2, cidx, intra, mode, qp, bypass, ctb_addr, cur_slice, cu_intra):
         """One decode_TU call; returns True when coefficients were coded."""
@@ -263,6 +318,8 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
         if intra:
             flags |= capi.TU_INTRA
             avail = avail_mask(x, y, nT, cidx, ctb_addr, cur_slice)
+            if no_bfilter_on_bypass and bypass:
+                flags |= capi.TU_NO_BOUNDARY_FILTER
         cbf = rng.random() < cbf_prob
         pos = lv = None
         if cbf:
@@ -273,7 +330,9 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
                 lv = np.clip(lv, -255, 255).astype(np.int16)
             elif log2 <= tskip_max_log2 and rng.random() < special_frac * 4:
                 flags |= capi.TU_TSKIP
-            if flags & (capi.TU_BYPASS | capi.TU_TSKIP):
+            if no_bfilter_on_bypass and intra and (flags & (capi.TU_BYPASS | capi.TU_TSKIP)) and mode in (10, 26):
+                flags |= capi.TU_RDPCM_H if mode == 10 else capi.TU_RDPCM_V  # implicit RDPCM (transform.cc:425-432)
+            elif flags & (capi.TU_BYPASS | capi.TU_TSKIP):
                 if rng.random() < rdpcm_frac:
                     flags |= capi.TU_RDPCM_H if rng.random() < 0.5 else capi.TU_RDPCM_V
                 if nT == 4 and cu_intra and rng.random() < rotate_frac:
@@ -303,6 +362,8 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
         cbf_l = tu_block(x, y, log2, 0, intra, lmode_of(x, y), qps[0], bypass, ctb_addr, cur_slice, intra)
         if cbf_l:
             nz[y >> 2:(y + size) >> 2, x >> 2:(x + size) >> 2] = True
+        if not chroma_format_idc:  # 4:0:0: no chroma TUs
+            return
         if log2 > 2:
             tu_block(x >> 1, y >> 1, log2 - 1, 1, intra, cmode, qps[1], bypass, ctb_addr, cur_slice, intra)
             tu_block(x >> 1, y >> 1, log2 - 1, 2, intra, cmode, qps[2], bypass, ctb_addr, cur_slice, intra)
@@ -318,6 +379,21 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
             return 4 * int(rng.integers(-16, 17)), 4 * int(rng.integers(-16, 17))  # integer position
         return int(rng.integers(-256, 257)), int(rng.integers(-256, 257))
 
+    def extreme_mv(pos, size, extent, pad, cpad):
+        """One MV component of a PU at `pos`: an int16 extreme, or the MC window (first tap: pos + int - 3 in luma,
+        pos / 2 + int - 1 in chroma) one sample before / on / after the rim of the slot's reference border, any phase."""
+        r = int(rng.integers(0, 6))
+        if r < 2:
+            return (-32768, 32767)[r]
+        side, d = int(rng.integers(0, 2)), int(rng.integers(-1, 2))
+        if r < 4:  # luma rims: -pad and extent + pad - 23 (the last window origin that fits)
+            t = (-pad if side == 0 else extent + pad - 23) + d
+            mv = 4 * (t + 3 - pos) + int(rng.integers(0, 4))
+        else:  # chroma rims: -cpad and extent / 2 + cpad - 11
+            t = (-cpad if side == 0 else extent // 2 + cpad - 11) + d
+            mv = 8 * (t + 1 - (pos >> 1)) + int(rng.integers(0, 8))
+        return int(np.clip(mv, -32768, 32767))
+
     def emit_pu(x, y, w, h):
         small = (w + h) == 12  # 8x4 / 4x8: uni-prediction only
         bi = pic_type == "B" and not small and rng.random() < 0.5
@@ -329,6 +405,8 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
             if rng.random() < 0.003:
                 ref[l] = -1  # missing reference -> mid-grey
             mv[l] = list(rand_mv())
+            if extreme_mv_frac and (x == 0 or y == 0 or x + w >= width or y + h >= height) and rng.random() < extreme_mv_frac:
+                mv[l] = [extreme_mv(x, w, width, _PAD_X, _PAD_CX), extreme_mv(y, h, height, _PAD_Y, _PAD_CY)]
         wt = 0
         if len(weights):
             flags |= capi.PU_WEIGHTED
@@ -347,14 +425,16 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
         qps = qp_primes(qpy)
         if bypass:
             nofilt[y >> 3:(y + size) >> 3, x >> 3:(x + size) >> 3] = 1
-        if intra and log2 <= 5 and rng.random() < special_frac:  # PCM CU (pcm_loop_filter_disable = 0 here)
+        if intra and log2 <= 5 and rng.random() < special_frac:  # PCM CU
             is_intra[y >> 2:(y + size) >> 2, x >> 2:(x + size) >> 2] = True
             tu_edge_v[y >> 2:(y + size) >> 2, x >> 2] = True
             tu_edge_h[y >> 2, x >> 2:(x + size) >> 2] = True
-            for c in range(3):
+            if pcm_lf_disable:  # the host folds pcm_loop_filter_disable into the no-filter map
+                nofilt[y >> 3:(y + size) >> 3, x >> 3:(x + size) >> 3] = 1
+            for c in range(3 if chroma_format_idc else 1):
                 s = size if c == 0 else size >> 1
                 n = s * s
-                lv = rng.integers(0, 1 << bit_depth, n).astype(np.int16)
+                lv = rng.integers(0, 1 << (bd_c if c else bit_depth), n).astype(np.int16)
                 emit_tu(x >> (1 if c else 0), y >> (1 if c else 0), log2 - (1 if c else 0), c, capi.TU_PCM, 0, 0, 0, np.arange(n, dtype=np.uint16), lv)
             return
         if intra:
@@ -465,20 +545,33 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
             b = np.where(ip | is_intra, 2, np.where(te & (nzp | nz), 1, np.where(~same | mvdiff, 1, 0)))
             b = np.where(edge, b, 0).astype(np.uint8)
             bs |= b if vertical else (b << 2)
+        if slice_deblock_off_frac:  # deblock.cc:215: a slice with deblocking off marks no edge of its CUs (the Q side)
+            off = (slices["flags"] & capi.SLICE_DEBLOCK_DISABLED) != 0
+            ys, xs = np.mgrid[0:h4, 0:w4]
+            bs[off[ctb_slice[((xs * 4) >> log2_ctb) + ((ys * 4) >> log2_ctb) * wctb]]] = 0
 
     # ---- SAO ----
     ctbs = np.zeros(n_ctb, CTB_DT)
     ctbs["slice_idx"] = ctb_slice
     ctbs["tile_id"] = ctb_tile
     if sao:
-        lim = 7 if bit_depth == 8 else 31
+        lim, lim_c = 7 if bit_depth == 8 else 31, 7 if bd_c == 8 else 31
         for i in range(n_ctb):
             tl, tc = int(rng.integers(0, 3)), int(rng.integers(0, 3))
             cl, cc = int(rng.integers(0, 4)), int(rng.integers(0, 4))
             ctbs[i]["sao_type"] = tl | (tc << 2) | (tc << 4)
             ctbs[i]["sao_eo_class"] = cl | (cc << 2) | (cc << 4)
             ctbs[i]["sao_band_pos"] = rng.integers(0, 32, 3)
-            off = rng.integers(-lim, lim + 1, (3, 4))
+            if lim == lim_c:
+                off = rng.integers(-lim, lim + 1, (3, 4))
+            else:
+                off = rng.integers(-np.array([[lim], [lim_c], [lim_c]]), np.array([[lim], [lim_c], [lim_c]]) + 1, (3, 4))
+            if sao_offset == "max":  # SaoOffsetVal at the largest magnitude the depth allows (sao_offset_abs << log2_sao_offset_scale)
+                for c, bd in enumerate((bit_depth, bd_c, bd_c)):
+                    mag = ((1 << (min(bd, 10) - 5)) - 1) << int(rng.integers(0, max(0, bd - 10) + 1))
+                    off[c] = np.where(off[c] < 0, -mag, mag)
+            else:
+                assert sao_offset == "random"
             for c, t in enumerate((tl, tc, tc)):
                 if t == 2:  # edge offsets: first two >= 0, last two <= 0
                     off[c] = [abs(off[c][0]), abs(off[c][1]), -abs(off[c][2]), -abs(off[c][3])]
@@ -488,13 +581,14 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
                         np.ascontiguousarray(qp_map.reshape(-1)), np.ascontiguousarray(nofilt.reshape(-1)), scaling)
 
 
-def random_planes(width, height, bit_depth, seed):
-    """Random reference picture (xorshift-like seeded noise with some smooth structure)."""
+def random_planes(width, height, bit_depth, seed, bit_depth_chroma=None, chroma_format_idc=1):
+    """Random reference picture (xorshift-like seeded noise with some smooth structure).  4:0:0: the luma plane only (the
+    same samples as the 4:2:0 picture's luma); chroma samples lie in [0, 2^bit_depth_chroma)."""
     rng = np.random.default_rng(seed)
     dt = np.uint16 if bit_depth > 8 else np.uint8
-    maxv = (1 << bit_depth) - 1
     planes = []
-    for c in range(3):
+    for c in range(3 if chroma_format_idc else 1):
+        maxv = (1 << (bit_depth if c == 0 or bit_depth_chroma is None else bit_depth_chroma)) - 1
         w, h = (width, height) if c == 0 else (width // 2, height // 2)
         base = rng.integers(0, maxv + 1, (h // 8 + 1, w // 8 + 1))
         img = np.kron(base, np.ones((8, 8), np.int64))[:h, :w] + rng.integers(-40, 41, (h, w))

@@ -1,6 +1,6 @@
 """Boundary B1 (include/b200hevc_dsp.h) on the GPU: every batched DSP-table entry against the REAL reference
 function (oracle/_ref/libref_shim.so -> the scalar table of libde265_ref.so), exercised the way the reference's
-dev-tools/test-*.cc exercise the SSE table: random blocks, all phases / modes / sizes, 8 and 10 bit.  Bit-exact.  Where oracle/_ref
+dev-tools/test-*.cc exercise the SSE table: random blocks, all phases / modes / sizes, 8, 9, 10 and 12 bit.  Bit-exact.  Where oracle/_ref
 is absent, the GPU's outputs are checked against digests of what the reference returned (tests/golden/ref_pins.json)."""
 import ctypes as C
 
@@ -41,7 +41,7 @@ def pix(rng, shape, bd, extreme=False):
     return a.astype(np.uint8 if bd == 8 else np.uint16)
 
 
-@pytest.mark.parametrize("bd", [8, 10])
+@pytest.mark.parametrize("bd", [8, 9, 10, 12])
 def test_mc_all_phases(ref, dsp, pins, bd):
     rng = np.random.default_rng(1)
     pt = u8p if bd == 8 else u16p
@@ -68,7 +68,7 @@ def test_mc_all_phases(ref, dsp, pins, bd):
         pins.check(got[:, :w], exp[:, :w], f"{'qpel' if luma else 'epel'} phase ({fx},{fy}) {w}x{h}")
 
 
-@pytest.mark.parametrize("bd", [8, 10])
+@pytest.mark.parametrize("bd", [8, 9, 10, 12])
 def test_weighted_prediction(ref, dsp, pins, bd):
     rng = np.random.default_rng(2)
     pt, suf = (u8p, "8") if bd == 8 else (u16p, "16")
@@ -93,7 +93,7 @@ def test_weighted_prediction(ref, dsp, pins, bd):
         pins.check(got[:, :w], exp[:, :w], f"{name} {w}x{h}")
 
 
-@pytest.mark.parametrize("bd", [8, 10])
+@pytest.mark.parametrize("bd", [8, 9, 10, 12])
 def test_transform_add(ref, dsp, pins, bd):
     rng = np.random.default_rng(3)
     pt, suf = (u8p, "8") if bd == 8 else (u16p, "16")
@@ -127,7 +127,7 @@ def test_transform_add(ref, dsp, pins, bd):
         pins.check(got, exp, name)
 
 
-@pytest.mark.parametrize("bd", [8, 10])
+@pytest.mark.parametrize("bd", [8, 9, 10, 12])
 def test_intra_prediction(ref, dsp, pins, bd):
     rng = np.random.default_rng(4)
     pt, suf = (u8p, "8") if bd == 8 else (u16p, "16")
@@ -149,7 +149,7 @@ def test_intra_prediction(ref, dsp, pins, bd):
         pins.check(got, exp, name)
 
 
-@pytest.mark.parametrize("bd", [8, 10])
+@pytest.mark.parametrize("bd", [8, 9, 10, 12])
 def test_deblock(ref, dsp, pins, bd):
     rng = np.random.default_rng(5)
     pt = u8p if bd == 8 else u16p

@@ -90,7 +90,7 @@ def test_idct_add(ref, orc, pins, log2, bd):
         pins.check(o, r)  # whole strided buffer, catches out-of-region writes
 
 
-@pytest.mark.parametrize("bd", [8, 10])
+@pytest.mark.parametrize("bd", [8, 9, 10, 12])
 def test_dst_add(ref, orc, pins, bd):
     stride = 21
     rng = np.random.default_rng(5)
@@ -130,7 +130,7 @@ def test_dequant(ref, orc, pins, log2):
 
 
 @pytest.mark.parametrize("log2", [2, 3, 4, 5])
-@pytest.mark.parametrize("bd", [8, 10])
+@pytest.mark.parametrize("bd", [8, 9, 10, 12])
 def test_transform_skip_and_bypass(ref, orc, pins, log2, bd):
     nT = 1 << log2
     stride = nT + 5
@@ -166,7 +166,7 @@ def _ref_plane(bd, w, h, seed, extreme):
     return rng.integers(0, maxv + 1, (h, w)).astype(np.uint16)
 
 
-@pytest.mark.parametrize("bd", [8, 10])
+@pytest.mark.parametrize("bd", [8, 9, 10, 12])
 @pytest.mark.parametrize("extreme", [False, True])
 def test_qpel_all_phases(ref, orc, pins, bd, extreme):
     W = H = 96
@@ -191,7 +191,7 @@ def test_qpel_all_phases(ref, orc, pins, bd, extreme):
                 pins.check(o[:, :w], r[:, :w], (w, h, xf, yf))
 
 
-@pytest.mark.parametrize("bd", [8, 10])
+@pytest.mark.parametrize("bd", [8, 9, 10, 12])
 def test_epel_all_phases(ref, orc, pins, bd):
     W = H = 64  # chroma plane size; luma picture = 128x128
     plane = _ref_plane(bd, W, H, 4321, False)
@@ -228,7 +228,7 @@ def test_mc_edge_clamping_matches_padded_reference(ref, orc, pins):
             pins.check(o[:, :w], r[:, :w], (x0, y0, xf, yf))
 
 
-@pytest.mark.parametrize("bd", [8, 10])
+@pytest.mark.parametrize("bd", [8, 9, 10, 12])
 def test_weighted_prediction(ref, orc, pins, bd):
     rng = np.random.default_rng(11)
     w, h, ss = 16, 6, 64
@@ -260,7 +260,7 @@ def test_weighted_prediction(ref, orc, pins, bd):
                  (P(s1, i16p), P(s2, i16p), C.c_ssize_t(ss), w, h, w1, o1s, w2, o2s, log2wd))
 
 
-@pytest.mark.parametrize("bd", [8, 10])
+@pytest.mark.parametrize("bd", [8, 9, 10, 12])
 def test_intra_all_modes(ref, orc, pins, bd):
     # all 35 modes x nT x cIdx x disableBoundaryFilter (dev-tools/test-intrapred.cc:163-177), + smoothing filter
     x = XorShift(0x1234ABCD)
@@ -297,7 +297,7 @@ def test_intra_all_modes(ref, orc, pins, bd):
                         pins.check(o, r, (nT, cidx, dis, mode))
 
 
-@pytest.mark.parametrize("bd", [8, 10])
+@pytest.mark.parametrize("bd", [8, 9, 10, 12])
 def test_deblock_segments(ref, orc, pins, bd):
     # all dE/dEp/dEq/filterP/filterQ combos x direction, tc in [1,25] (dev-tools/test-deblk.cc:94-109) + chroma
     x = XorShift(0xDEB10C)
