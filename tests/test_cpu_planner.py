@@ -28,7 +28,8 @@ def plan(lib, pic, region=16):
     return dict(units=units[:c[0]], la=la[:c[1]], n_aw=c[2], n_a8=c[3], lb=lb[:c[4]], ts=ts[:c[5] + 1] if c[5] else ts[:0], ref_mask=c[6])
 
 
-def check_picture(lib, pic):
+def check_picture(lib, pic, region=16):
+    """`region`: the luma size of an intra region task the planner was run with (B200_REGION)."""
     r = plan(lib, pic)
     tus, pus = pic.tus, pic.pus
     flags = tus["flags"].astype(int)
@@ -82,17 +83,17 @@ def check_picture(lib, pic):
         if len(set(planes)) > 1:
             assert merged
             n_merged += 1
-        rx0, ry0 = (int(tus["x"][members[0]]) << (1 if planes[0] else 0)) // 16, (int(tus["y"][members[0]]) << (1 if planes[0] else 0)) // 16
+        rx0, ry0 = (int(tus["x"][members[0]]) << (1 if planes[0] else 0)) // region, (int(tus["y"][members[0]]) << (1 if planes[0] else 0)) // region
         for c0 in sorted(set(planes)):
             seg = np.array([i for i in members if int(tus["cidx"][i]) == c0])
-            G = 16 >> (1 if c0 else 0)
+            G = region >> (1 if c0 else 0)
             assert (np.diff(seg.astype(np.int64)) > 0).all(), "decode order inside a plane of a task"
             for i in seg:
                 tu = tus[i]
                 nT = 1 << int(tu["log2_size"])
                 if len(members) > 1:
                     sh = 1 if c0 else 0
-                    assert nT < G and (int(tu["x"]) << sh) // 16 == rx0 and (int(tu["y"]) << sh) // 16 == ry0
+                    assert nT < G and (int(tu["x"]) << sh) // region == rx0 and (int(tu["y"]) << sh) // region == ry0
                 task_of[int(i)] = t
                 owner[c0][int(tu["y"]) // 4:(int(tu["y"]) + nT) // 4, int(tu["x"]) // 4:(int(tu["x"]) + nT) // 4] = t
     assert merged or n_merged == 0
@@ -115,14 +116,36 @@ def check_picture(lib, pic):
     return len(ts) - 1
 
 
-@pytest.mark.parametrize("kind,size,kw", [("I", (256, 192), {}), ("I", (200, 136), {}), ("B", (320, 192), {}), ("P", (256, 128), dict(special_frac=0.15)),
-                                          ("I", (192, 128), dict(log2_ctb=4, size_area=(0.0, 0.0, 0.4, 0.6))), ("I", (192, 128), dict(log2_ctb=5, size_area=(0.0, 0.3, 0.4, 0.3)))])
+PLANNER_CASES = [("I", (256, 192), {}), ("I", (200, 136), {}), ("B", (320, 192), {}), ("P", (256, 128), dict(special_frac=0.15)),
+                 ("I", (192, 128), dict(log2_ctb=4, size_area=(0.0, 0.0, 0.4, 0.6))), ("I", (192, 128), dict(log2_ctb=5, size_area=(0.0, 0.3, 0.4, 0.3)))]
+
+
+@pytest.mark.parametrize("kind,size,kw", PLANNER_CASES)
 def test_planner_work_lists(b200lib, kind, size, kw):
     refs = {} if kind == "I" else dict(ref_slots=(0, 1) if kind == "B" else (0,))
     pic = synth.make_picture(size[0], size[1], kind, seed=77, dst_slot=2, **refs, **kw)
     n_tasks = check_picture(b200lib, pic)
     if kind == "I":
         assert n_tasks > 0
+
+
+@pytest.mark.parametrize("env", [{"B200_REGION": "8"}, {"B200_INTRA_ORDER": "level_i"}, {"B200_INTRA_ORDER": "diag"},
+                                 {"B200_REGION": "8", "B200_INTRA_ORDER": "diag"}], ids=lambda e: "-".join(f"{k[5:].lower()}={v}" for k, v in e.items()))
+@pytest.mark.parametrize("kind,size,kw", PLANNER_CASES)
+def test_planner_work_lists_other_task_shapes(b200lib, monkeypatch, env, kind, size, kw):
+    """The intra task shapes and ticket orders the engine can be switched to (b200_plan_picture_host reads B200_REGION and
+    B200_INTRA_ORDER like b200_engine_create): 8x8-luma regions, and the per-TU level order and CTB anti-diagonal order next
+    to the default region-level order.  The same membership and topological-order properties must hold."""
+    for k, v in env.items():
+        monkeypatch.setenv(k, v)
+    refs = {} if kind == "I" else dict(ref_slots=(0, 1) if kind == "B" else (0,))
+    pic = synth.make_picture(size[0], size[1], kind, seed=77, dst_slot=2, **refs, **kw)
+    n_tasks = check_picture(b200lib, pic, region=int(env.get("B200_REGION", 16)))
+    if kind == "I":
+        assert n_tasks > 0
+    if env.get("B200_REGION") == "8" and kind == "I":  # the switch took effect: smaller regions, more tasks than with 16x16 regions
+        monkeypatch.delenv("B200_REGION")
+        assert n_tasks > check_picture(b200lib, pic)
 
 
 def test_planner_rejects_malformed_records(b200lib):
