@@ -327,31 +327,92 @@ __device__ __forceinline__ void tu_intra_small(const b200_tu& tu, P* dst, int ts
   __syncwarp();
 }
 
+// Substitution by clamping applicable?  When the left column, the corner and the top row of the TU itself are available
+// (every TU that does not touch a picture / slice / tile boundary or a constrained-intra hole) and the bottom-left and
+// top-right reach are each available up to some point and not beyond, the available border samples are one interval
+// [lo, hi] of border indices and the substitution process (intrapred.h:637-674) degenerates to clamping the index into it:
+// a missing bottom-left part repeats border[lo], a missing top-right part repeats border[hi].  -2nT <= lo <= -nT, nT <= hi <= 2nT.
+__device__ __forceinline__ bool intra_border_clamps(const b200_tu& tu, int& lo, int& hi)
+{
+  const int q = 1 << (tu.log2_size - 2);  // groups of 4 samples per side
+  const uint64_t g = (1ull << q) - 1, av = tu.avail;
+  if ((av & g) != g || !((av >> B200_AVAIL_CORNER_BIT) & 1) || ((av >> B200_AVAIL_TOP_BIT0) & g) != g) return false;
+  const unsigned bl = (unsigned)((av >> q) & g), tr = (unsigned)((av >> (B200_AVAIL_TOP_BIT0 + q)) & g);
+  if ((bl & (bl + 1)) || (tr & (tr + 1))) return false;  // available groups must start at the inner end and not resume
+  lo = -4 * (q + __popc(bl));
+  hi = 4 * (q + __popc(tr));
+  return true;
+}
+
+// -------------------------------------------------------------------------------------------------
+// What the region loop needs of a small TU, decoded from its record before the task waits for its neighbours: lane i
+// holds TU i's descriptor and the dependent TU loop fetches it with two shuffles (no shared-memory record load, no
+// constant-table lookup on the chain).
+//   a: [0,10) offset in the region tile | [10,16) intra mode | 16 nT == 8 | 17 fast path applies | 18 [1 2 1] smoothing |
+//      19 boundary filter of modes 10 / 26 | 20 luma (DC edge filter) | 21 CBF | [22,32) residual base in res[]
+//   b: [0,8) angle (int8) | [8,21) -inverse angle | fast path only: [21,23) -lo2 / 4 - 1 | [23,25) hi2 / 4 - 1, the clamps of
+//      the border index that reproduce the substitution (lo2 <= -nT, hi2 >= nT)
+// -------------------------------------------------------------------------------------------------
+struct TuDesc {
+  uint32_t a, b;
+  __device__ __forceinline__ int toff() const { return a & 1023; }
+  __device__ __forceinline__ int mode() const { return (a >> 10) & 63; }
+  __device__ __forceinline__ bool big() const { return (a >> 16) & 1; }
+  __device__ __forceinline__ bool fast() const { return (a >> 17) & 1; }
+  __device__ __forceinline__ bool smooth() const { return (a >> 18) & 1; }
+  __device__ __forceinline__ bool bfilt() const { return (a >> 19) & 1; }
+  __device__ __forceinline__ bool luma() const { return (a >> 20) & 1; }
+  __device__ __forceinline__ bool cbf() const { return (a >> 21) & 1; }
+  __device__ __forceinline__ int rbase() const { return a >> 22; }
+  __device__ __forceinline__ int angle() const { return (int)(int8_t)(b & 255); }
+  __device__ __forceinline__ int inv() const { return -(int)((b >> 8) & 8191); }
+  __device__ __forceinline__ int lo2() const { return -4 * (int)(((b >> 21) & 3) + 1); }
+  __device__ __forceinline__ int hi2() const { return 4 * (int)(((b >> 23) & 3) + 1); }
+};
+
+__device__ __forceinline__ TuDesc tu_desc(const b200_tu& tu, int G, bool filter_plane, int rbase)
+{
+  const int nT = 1 << tu.log2_size, mode = tu.intra_mode;
+  int lo2 = 0, hi2 = 0;
+  const bool fast = intra_border_clamps(tu, lo2, hi2);
+  const bool smooth = nT == 8 && filter_plane && mode != 1 && min(abs(mode - 26), abs(mode - 10)) > 7;
+  const bool bfilt = tu.cidx == 0 && !(tu.flags & B200_TU_NO_BOUNDARY_FILTER) && (mode == 26 || mode == 10);
+  const int angle = (mode >= 2) ? k_intra_angle[mode] : 0;
+  const int inv = (angle < 0) ? (int)k_inv_angle[mode - 11] : 0;
+  TuDesc d;
+  d.a = (uint32_t)((tu.y & (G - 1)) * RC_TILE_STRIDE + (tu.x & (G - 1))) | (uint32_t)mode << 10 | (uint32_t)(nT == 8) << 16 | (uint32_t)fast << 17 |
+        (uint32_t)smooth << 18 | (uint32_t)bfilt << 19 | (uint32_t)(tu.cidx == 0) << 20 | (uint32_t)((tu.flags & B200_TU_CBF) != 0) << 21 |
+        (uint32_t)rbase << 22;
+  d.b = (uint32_t)(angle & 255) | (uint32_t)(-inv) << 8;
+  if (fast) d.b |= (uint32_t)(-lo2 / 4 - 1) << 21 | (uint32_t)(hi2 / 4 - 1) << 23;
+  return d;
+}
+
+__device__ __forceinline__ TuDesc shfl_desc(const TuDesc& d, int src)
+{
+  return TuDesc{__shfl_sync(RC_FULL, d.a, src), __shfl_sync(RC_FULL, d.b, src)};
+}
+
 // -------------------------------------------------------------------------------------------------
 // Fast path of the small TUs: when the left column, the corner and the top row of the TU are all available (every TU
 // that does not touch a picture / slice / tile boundary or a constrained-intra hole), the substitution process
 // (intrapred.h:637-674) degenerates to index clamping: a missing bottom-left part repeats border[-nT], a missing
 // top-right part repeats border[nT].  Every lane then reads the border samples its pixels need straight from the
 // shared-memory tile (no gather, ballot or shuffle chain); the [1 2 1] smoothing of 8x8 luma TUs is applied on the fly.
-// This is the dependent part of the intra DAG, so what counts is its latency: ~50 mostly independent instructions.
+// This is the dependent part of the intra DAG, so what counts is its latency: the parameters come decoded (TuDesc) and
+// the residual r[] was loaded from shared memory before the prediction, next to the border reads.
 // -------------------------------------------------------------------------------------------------
 template <typename P, int LOG2>
-__device__ __forceinline__ void tu_intra_fast(const b200_tu& tu, P* dst, int ts, int bd, bool filter_plane, const res_t* res, int lane)
+__device__ __forceinline__ void tu_intra_fast(const TuDesc& d, P* dst, int ts, int bd, const int (&r)[2], int lane)
 {
   constexpr int nT = 1 << LOG2;
-  const int mode = tu.intra_mode, cidx = tu.cidx;
-  const uint64_t avail = tu.avail;
-  const int lo = ((avail >> (nT / 4)) & 1) ? -2 * nT : -nT;                          // first bottom-left group available?
-  const int hi = ((avail >> (B200_AVAIL_TOP_BIT0 + nT / 4)) & 1) ? 2 * nT : nT;      // first top-right group available?
-  // (groups are 4 samples; for nT == 8 the second bottom-left / top-right group may be missing on its own)
-  const int lo2 = (nT == 8 && lo < -nT && !((avail >> 3) & 1)) ? -12 : lo;
-  const int hi2 = (nT == 8 && hi > nT && !((avail >> (B200_AVAIL_TOP_BIT0 + 3)) & 1)) ? 12 : hi;
+  const int mode = d.mode();
+  const int lo2 = d.lo2(), hi2 = d.hi2();
   auto S = [&](int i) -> int {  // substituted border sample
     i = min(max(i, lo2), hi2);
     return (int)dst[(i < 0) ? (-i - 1) * ts - 1 : i - 1 - ts];
   };
-  bool smooth = false;
-  if (nT == 8 && filter_plane && mode != 1) smooth = min(abs(mode - 26), abs(mode - 10)) > 7;
+  const bool smooth = nT == 8 && d.smooth();
   auto B = [&](int i) -> int {  // border sample after the optional smoothing (intrapred.h:185-258)
     if (nT == 8 && smooth && i > -2 * nT && i < 2 * nT) return (S(i - 1) + 2 * S(i) + S(i + 1) + 2) >> 2;
     return S(i);
@@ -373,7 +434,7 @@ __device__ __forceinline__ void tu_intra_fast(const b200_tu& tu, P* dst, int ts,
     for (int p = 0; p < NP; p++) {
       const int o = lane + 32 * p, x = o & (nT - 1), y = (o >> LOG2) & (nT - 1);
       int v = dc;
-      if (cidx == 0) {
+      if (d.luma()) {
         if (x == 0 && y == 0) v = (S(-1) + 2 * dc + S(1) + 2) >> 2;
         else if (y == 0) v = (S(x + 1) + 3 * dc + 2) >> 2;
         else if (x == 0) v = (S(-y - 1) + 3 * dc + 2) >> 2;
@@ -381,11 +442,11 @@ __device__ __forceinline__ void tu_intra_fast(const b200_tu& tu, P* dst, int ts,
       px[p] = v;
     }
   } else {  // angular, intrapred.h:330-433
-    const int angle = k_intra_angle[mode];
+    const int angle = d.angle();
     const bool vert = mode >= 18;
     const int sgn = vert ? 1 : -1;
-    const int inv = (angle < 0) ? (int)k_inv_angle[mode - 11] : 0;
-    const bool bfilt = (cidx == 0 && !(tu.flags & B200_TU_NO_BOUNDARY_FILTER) && (mode == 26 || mode == 10));
+    const int inv = d.inv();
+    const bool bfilt = d.bfilt();
     // ref[k] = border[sgn*k] for k >= 0, border[-sgn*((k*inv+128)>>8)] for the projected part k < 0
     auto R = [&](int k) -> int { return B(k >= 0 ? sgn * k : -sgn * ((k * inv + 128) >> 8)); };
 #pragma unroll
@@ -402,32 +463,14 @@ __device__ __forceinline__ void tu_intra_fast(const b200_tu& tu, P* dst, int ts,
       px[p] = v;
     }
   }
-  __syncwarp();  // all border reads done before the block is overwritten (the border does not overlap the block, but keeps the
-                 // read/write phases of consecutive TUs apart)
+  // No barrier between the border reads and the block writes: the border (column -1, row -1) never overlaps the TU's own
+  // block, and the barrier after the writes orders them before the next TU's reads.
 #pragma unroll
   for (int p = 0; p < NP; p++) {
     const int o = lane + 32 * p, x = o & (nT - 1), y = (o >> LOG2) & (nT - 1);
-    if (o < nT * nT) {
-      int v = px[p];
-      if (res) v = clip_bd(v + res[o], bd);
-      dst[x + y * ts] = (P)v;
-    }
+    if (o < nT * nT) dst[x + y * ts] = (P)clip_bd(px[p] + r[p], bd);  // r = 0 without a residual: px is already in range
   }
   __syncwarp();
-}
-
-// fast path applicable?  left column, corner and top row (of the TU itself) available
-__device__ __forceinline__ bool intra_fast_ok(const b200_tu& tu)
-{
-  const int g = 1 << (tu.log2_size - 2);  // groups of 4 samples per side
-  const uint64_t need = ((1ull << g) - 1) | (1ull << B200_AVAIL_CORNER_BIT) | (((1ull << g) - 1) << B200_AVAIL_TOP_BIT0);
-  if ((tu.avail & need) != need) return false;
-  if (g == 2) {  // 8x8: the outer bottom-left / top-right group must not be available without the inner one (clamping
-                 // reproduces the substitution only for availability that ends once)
-    const unsigned bl = (unsigned)(tu.avail >> 2) & 3, tr = (unsigned)(tu.avail >> (B200_AVAIL_TOP_BIT0 + 2)) & 3;
-    if (bl == 2 || tr == 2) return false;
-  }
-  return true;
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -571,6 +614,137 @@ __device__ void tu_intra_large(const b200_tu& tu, const P* gsrc, int gstride, P*
     }
   }
   __syncwarp();
+}
+
+// -------------------------------------------------------------------------------------------------
+// Large TU (nT = 16 or 32) whose border substitution is a clamp (intra_border_clamps: every such TU away from the picture /
+// slice / tile edges), fused: each lane loads the (clamped) border samples it owns, no ballot / shuffle substitution chain,
+// the smoothing on registers, ONE shared-memory write of the final border, then prediction + residual straight to the
+// picture, 4 horizontally adjacent samples per lane and store; the angular reference array is not built, its index mapping
+// is applied on each read (as in tu_intra_fast).  The general path (tu_intra_large, residual add, block_store) has a
+// barrier between each of those phases.
+// gdst = the TU's top-left sample in the picture (row stride gstride), res = its residual (row stride nT) or nullptr.
+// -------------------------------------------------------------------------------------------------
+template <typename P>
+__device__ void tu_intra_large_clamped(const b200_tu& tu, int lo, int hi, P* gdst, int gstride, int bd, int bd_luma, uint32_t pic_flags,
+                                       bool filter_plane, const res_t* res, P* bmem, int lane)
+{
+  const int log2 = tu.log2_size, nT = 1 << log2, mode = tu.intra_mode, cidx = tu.cidx;
+  const int total = 4 * nT + 1;
+  P* bs = bmem + 2 * 32 + 2;  // centre element; valid [-2nT, 2nT]
+  // ---- gather + substitution: scan index s = 32 * c5 + lane, border[s - 2nT] ----
+  constexpr int MAXC = 5;
+  int v[MAXC];
+#pragma unroll
+  for (int c5 = 0; c5 < MAXC; c5++) {
+    const int s = 32 * c5 + lane, i = min(max(s - 2 * nT, lo), hi);
+    v[c5] = 0;
+    if (s < total) v[c5] = (int)__ldcg(i < 0 ? gdst - 1 + (-i - 1) * gstride : gdst + (i - 1) - gstride);
+  }
+  // ---- smoothing (intrapred.h:185-258) on registers, then the border to shared memory ----
+  const bool filt = filter_plane && mode != 1 && min(abs(mode - 26), abs(mode - 10)) > ((nT == 16) ? 1 : 0);
+  bool strong = false;
+  int c0 = 0, bl = 0, tr = 0;  // border[0], border[-64], border[64] of a 32x32 TU
+  if (filt && (pic_flags & B200_PIC_STRONG_INTRA_SMOOTHING) && cidx == 0 && nT == 32) {
+    bl = __shfl_sync(RC_FULL, v[0], 0);
+    const int ml = __shfl_sync(RC_FULL, v[1], 0);
+    c0 = __shfl_sync(RC_FULL, v[2], 0);
+    const int mt = __shfl_sync(RC_FULL, v[3], 0);
+    tr = __shfl_sync(RC_FULL, v[4], 0);
+    strong = abs(c0 + tr - 2 * mt) < (1 << (bd_luma - 5)) && abs(c0 + bl - 2 * ml) < (1 << (bd_luma - 5));
+  }
+#pragma unroll
+  for (int c5 = 0; c5 < MAXC; c5++) {
+    if (32 * c5 < total) {  // warp-uniform
+      const int s = 32 * c5 + lane, i = s - 2 * nT;
+      int f = v[c5];
+      if (filt) {
+        int vm = __shfl_up_sync(RC_FULL, v[c5], 1), vp = __shfl_down_sync(RC_FULL, v[c5], 1);
+        const int vm_prev = (c5 > 0) ? __shfl_sync(RC_FULL, v[c5 > 0 ? c5 - 1 : 0], 31) : 0;
+        const int vp_next = (c5 + 1 < MAXC) ? __shfl_sync(RC_FULL, v[c5 + 1 < MAXC ? c5 + 1 : c5], 0) : 0;
+        if (lane == 0) vm = vm_prev;
+        if (lane == 31) vp = vp_next;
+        if (i == -2 * nT || i == 2 * nT) f = v[c5];
+        else if (strong) f = (i == 0) ? c0 : (i < 0) ? c0 + (((-i) * (bl - c0) + 32) >> 6) : c0 + ((i * (tr - c0) + 32) >> 6);
+        else f = (vp + 2 * v[c5] + vm + 2) >> 2;
+      }
+      if (s < total) bs[i] = (P)f;
+    }
+  }
+  __syncwarp();
+  // ---- prediction + residual, 4 samples per lane and group (intrapred.h:261-433) ----
+  auto emit = [&](int x, int y, int (&p)[4]) {
+    if (res) {
+      const uint2 rw = *reinterpret_cast<const uint2*>(res + x + (y << log2));
+      p[0] += (int)(int16_t)(rw.x & 0xffff);
+      p[1] += (int)(int16_t)(rw.x >> 16);
+      p[2] += (int)(int16_t)(rw.y & 0xffff);
+      p[3] += (int)(int16_t)(rw.y >> 16);
+    }
+#pragma unroll
+    for (int k = 0; k < 4; k++) p[k] = clip_bd(p[k], bd);  // (a prediction alone is in range)
+    P* d = gdst + (size_t)y * gstride + x;
+    if (sizeof(P) == 1) *reinterpret_cast<uint32_t*>(d) = (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24;
+    else *reinterpret_cast<uint2*>(d) = make_uint2((uint32_t)p[0] | (uint32_t)p[1] << 16, (uint32_t)p[2] | (uint32_t)p[3] << 16);
+  };
+  const int ngroups = nT * nT / 4;  // 64 or 256: 2 or 8 per lane
+  if (mode == 0) {
+    const int trv = bs[1 + nT], blv = bs[-1 - nT];
+    for (int g = lane; g < ngroups; g += 32) {
+      const int x = (g & (nT / 4 - 1)) * 4, y = g >> (log2 - 2);
+      const int l = bs[-1 - y];
+      int p[4];
+#pragma unroll
+      for (int k = 0; k < 4; k++)
+        p[k] = ((nT - 1 - x - k) * l + (x + k + 1) * trv + (nT - 1 - y) * (int)bs[1 + x + k] + (y + 1) * blv + nT) >> (log2 + 1);
+      emit(x, y, p);
+    }
+  } else if (mode == 1) {
+    const int part = (lane < nT) ? (int)bs[lane + 1] + (int)bs[-lane - 1] : 0;
+    const int dc = (__reduce_add_sync(RC_FULL, part) + nT) >> (log2 + 1);
+    const bool edge = (cidx == 0 && nT < 32);
+    for (int g = lane; g < ngroups; g += 32) {
+      const int x = (g & (nT / 4 - 1)) * 4, y = g >> (log2 - 2);
+      int p[4];
+#pragma unroll
+      for (int k = 0; k < 4; k++) {
+        int vv = dc;
+        if (edge) {
+          if (x + k == 0 && y == 0) vv = ((int)bs[-1] + 2 * dc + (int)bs[1] + 2) >> 2;
+          else if (y == 0) vv = ((int)bs[x + k + 1] + 3 * dc + 2) >> 2;
+          else if (x + k == 0) vv = ((int)bs[-y - 1] + 3 * dc + 2) >> 2;
+        }
+        p[k] = vv;
+      }
+      emit(x, y, p);
+    }
+  } else {
+    const int angle = k_intra_angle[mode];
+    const bool vert = mode >= 18;
+    const int sgn = vert ? 1 : -1;
+    const int inv = (angle < 0) ? (int)k_inv_angle[mode - 11] : 0;
+    const bool bfilt = (cidx == 0 && nT < 32 && !(tu.flags & B200_TU_NO_BOUNDARY_FILTER) && (mode == 26 || mode == 10));
+    // ref[k] = border[sgn*k] for k >= 0, border[-sgn*((k*inv+128)>>8)] for the projected part k < 0 (intrapred.h:352-364,392-404);
+    // k <= 2nT + 1, and 2nT + 1 only where the interpolation weight of that sample is 0
+    auto R = [&](int k) -> int { return bs[k >= 0 ? sgn * min(k, 2 * nT) : -sgn * ((k * inv + 128) >> 8)]; };
+    for (int g = lane; g < ngroups; g += 32) {
+      const int x = (g & (nT / 4 - 1)) * 4, y = g >> (log2 - 2);
+      int p[4];
+#pragma unroll
+      for (int k = 0; k < 4; k++) {
+        const int a = vert ? y : x + k, b = vert ? x + k : y;
+        const int idx = ((a + 1) * angle) >> 5, fact = ((a + 1) * angle) & 31;
+        const int r1 = R(b + idx + 1), r2 = R(b + idx + 2);
+        int vv = ((32 - fact) * r1 + fact * r2 + 16) >> 5;
+        if (bfilt) {
+          if (mode == 26 && x + k == 0) vv = clip_bd((int)bs[1] + (((int)bs[-1 - y] - (int)bs[0]) >> 1), bd);
+          if (mode == 10 && y == 0) vv = clip_bd((int)bs[-1] + (((int)bs[1 + x + k] - (int)bs[0]) >> 1), bd);
+        }
+        p[k] = vv;
+      }
+      emit(x, y, p);
+    }
+  }
 }
 
 // TU block -> picture plane, 4-byte units (TU rows are 4-byte aligned: x multiple of 4 samples)
@@ -734,6 +908,7 @@ __global__ void __launch_bounds__(RC_THREADS, 3) k_intra(DevPic pic, ReconArgs a
       const int mc = (lane < (int)count) ? tus[lane].cidx : -1, pc = (lane > 0 && lane < (int)count) ? tus[lane - 1].cidx : -1;
       seg_starts = __ballot_sync(RC_FULL, lane < (int)count && (lane == 0 || mc != pc));
     }
+    TuDesc desc{0u, 0u};  // region tasks: lane i < count holds TU i's descriptor
     {
       // residuals of all the task's TUs, in parallel where the sizes allow: lane i owns TU i's record; 4x4 TUs run one
       // per lane, 8x8 TUs one per quarter-warp, larger ones one after the other on the whole warp.  res holds the TUs'
@@ -749,6 +924,10 @@ __global__ void __launch_bounds__(RC_THREADS, 3) k_intra(DevPic pic, ReconArgs a
         if (lane >= d) incl += up;
       }
       const int my_rbase = incl - sz;
+      if (region && mine) {
+        const int c = mytu.cidx;
+        desc = tu_desc(mytu, args.region >> (c ? 1 : 0), !(pic.flags & B200_PIC_INTRA_SMOOTHING_OFF) && (c == 0 || pic.chroma == 3), my_rbase);
+      }
       const bool cbf = mine && (mytu.flags & B200_TU_CBF);
       const unsigned m8 = __ballot_sync(RC_FULL, cbf && l2 == 3), mw = __ballot_sync(RC_FULL, cbf && l2 > 3);
       uint32_t* scratch = reinterpret_cast<uint32_t*>(sm.coef[warp]);
@@ -835,17 +1014,23 @@ __global__ void __launch_bounds__(RC_THREADS, 3) k_intra(DevPic pic, ReconArgs a
       const bool filter_plane = !(pic.flags & B200_PIC_INTRA_SMOOTHING_OFF) && (c == 0 || pic.chroma == 3);
       const int nT = 1 << tu0.log2_size;
       const int gstride = pic.pitch[c] / (int)sizeof(P);
-      const P* gsrc = row_ptr<P>(pic.cur[c], pic.pitch[c], tu0.y) + tu0.x;
-      tu_intra_large<P>(tu0, gsrc, gstride, blk, bd, pic.bd_y, pic.flags, filter_plane, sm.border[warp][0], sm.border[warp][1], lane);
-      if (tu0.flags & B200_TU_CBF) {
-        for (int o = lane; o < nT * nT; o += 32) blk[o] = (P)clip_bd((int)blk[o] + res[o], bd);
-        __syncwarp();
+      P* gdst = row_ptr<P>(pic.cur[c], pic.pitch[c], tu0.y) + tu0.x;
+      int lo = 0, hi = 0;
+      if (nT >= 16 && intra_border_clamps(tu0, lo, hi)) {
+        tu_intra_large_clamped<P>(tu0, lo, hi, gdst, gstride, bd, pic.bd_y, pic.flags, filter_plane, (tu0.flags & B200_TU_CBF) ? res : nullptr,
+                                  sm.border[warp][0], lane);
+        tr_cycles(6);  // gather and store are inside: counted with the prediction
+      } else {
+        tu_intra_large<P>(tu0, gdst, gstride, blk, bd, pic.bd_y, pic.flags, filter_plane, sm.border[warp][0], sm.border[warp][1], lane);
+        if (tu0.flags & B200_TU_CBF) {
+          for (int o = lane; o < nT * nT; o += 32) blk[o] = (P)clip_bd((int)blk[o] + res[o], bd);
+          __syncwarp();
+        }
+        tr_cycles(6);  // the border gather is inside tu_intra_large: counted with the prediction
+        block_store<P>(blk, pic.cur[c], pic.pitch[c], tu0.x, tu0.y, nT, lane);
       }
-      tr_cycles(6);  // the border gather is inside tu_intra_large: counted with the prediction
-      block_store<P>(blk, pic.cur[c], pic.pitch[c], tu0.x, tu0.y, nT, lane);
     } else {
       // ---- regions of small TUs: stage region + top row (2G) + left column (2G) in shared memory, run the TUs in order ----
-      int rbase = 0;
       for (unsigned ss = seg_starts; ss; ss &= ss - 1) {
         const int s0 = __ffs(ss) - 1, s1 = (ss & (ss - 1)) ? __ffs(ss & (ss - 1)) - 1 : (int)count;
         const b200_tu& ts0 = tus[s0];
@@ -901,14 +1086,25 @@ __global__ void __launch_bounds__(RC_THREADS, 3) k_intra(DevPic pic, ReconArgs a
         if (left) tile[lane * TS - 1] = left_s;
         __syncwarp();
         tr_cycles(5);
+        TuDesc d = shfl_desc(desc, s0);
         for (int i = s0; i < s1; i++) {
-          const b200_tu& tu = tus[i];
-          P* tdst = tile + (tu.y - ry) * TS + (tu.x - rx);
-          const res_t* tres = (tu.flags & B200_TU_CBF) ? res + rbase : nullptr;
-          if (!intra_fast_ok(tu)) tu_intra_small<P>(tu, tdst, TS, bd, filter_plane, tres, lane);
-          else if (tu.log2_size == 2) tu_intra_fast<P, 2>(tu, tdst, TS, bd, filter_plane, tres, lane);
-          else tu_intra_fast<P, 3>(tu, tdst, TS, bd, filter_plane, tres, lane);
-          rbase += 1 << (2 * tu.log2_size);
+          const TuDesc dn = shfl_desc(desc, (i + 1) & 31);  // the next TU's, off the chain
+          P* tdst = tile + d.toff();
+          const res_t* tres = d.cbf() ? res + d.rbase() : nullptr;
+          if (!d.fast()) {
+            tu_intra_small<P>(tus[i], tdst, TS, bd, filter_plane, tres, lane);
+          } else {
+            // the residual is read next to the border samples, not after the prediction
+            const int n = d.big() ? 64 : 16;
+            int r[2] = {0, 0};
+            if (tres) {
+              if (lane < n) r[0] = tres[lane];
+              if (lane + 32 < n) r[1] = tres[lane + 32];
+            }
+            if (d.big()) tu_intra_fast<P, 3>(d, tdst, TS, bd, r, lane);
+            else tu_intra_fast<P, 2>(d, tdst, TS, bd, r, lane);
+          }
+          d = dn;
         }
         tr_cycles(6);
         if (full) {  // whole rows as 4-byte words (tile rows are 4-byte aligned: TS * sizeof(P) and the origin offset are multiples of 4)
