@@ -95,7 +95,7 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
                  rdpcm_frac=0.0, rotate_frac=0.0, tskip_max_log2=2, chroma_format_idc=1, bit_depth_chroma=None, chroma_qp_offsets=None,
                  lf_offsets=None, weight_range="narrow", sao_offset="random", extreme_mv_frac=0.0, strong_smoothing=True,
                  intra_smoothing_off=False, no_bfilter_on_bypass=False, pcm_lf_disable=False, slice_deblock_off_frac=0.0,
-                 slice_sao_off_frac=0.0, skip_sao=False):
+                 slice_sao_off_frac=0.0, skip_sao=False, constrained_intra=False):
     """Generate one picture.  ``size_area`` = fraction of the picture area coded as 64/32/16/8 CUs.
     ``tiles`` = (columns, rows) of uniformly spaced tiles (pps.cc uniform_spacing rule): CTBs are then coded in tile-scan
     order and intra availability stops at tile borders (intrapred.h:488-503); ``lf_across_tiles`` False also removes the
@@ -117,7 +117,9 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
     intra TUs of bypass CUs, implicit RDPCM on their horizontal / vertical bypass and transform-skip TUs, as
     integration/libde265_hooks.cc records them); ``pcm_lf_disable``: pcm_loop_filter_disable (PCM CUs in ``nofilt_map``);
     ``slice_deblock_off_frac`` / ``slice_sao_off_frac``: share of the slices with deblocking off (their edges get bS 0) resp.
-    each SAO plane flag off; ``skip_sao``: PIC_SKIP_SAO."""
+    each SAO plane flag off; ``skip_sao``: PIC_SKIP_SAO; ``constrained_intra``: constrained_intra_pred_flag, a neighbour group
+    of an intra TU counts as available only if its CU is intra (intrapred.h:557-616, as integration/libde265_hooks.cc records
+    it): only the ``avail`` masks change."""
     assert width % 8 == 0 and height % 8 == 0
     assert chroma_format_idc in (0, 1)
     rng = np.random.default_rng(seed)
@@ -277,7 +279,9 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
             ca = (xn >> log2_ctb) + (yn >> log2_ctb) * wctb
             if ctb_slice[ca] != cur_slice or ctb_tile[ca] != ctb_tile[ctb_addr]:
                 return False
-            return (int(ts_of[ca]) << 8) + int(_Z[(yn & (S - 1)) >> 2, (xn & (S - 1)) >> 2]) <= cur_z
+            if (int(ts_of[ca]) << 8) + int(_Z[(yn & (S - 1)) >> 2, (xn & (S - 1)) >> 2]) > cur_z:
+                return False
+            return not constrained_intra or bool(is_intra[yn >> 2, xn >> 2])
 
         m = 0
         n_bottom = min(2 * nT, ((height - (yB << sh)) + sh) >> sh)

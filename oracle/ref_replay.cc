@@ -49,6 +49,13 @@ struct Replay : public base_context {
   de265_image* slot[B200_MAX_SLOTS] = {};
   std::unique_ptr<thread_context> tctx;
   slice_segment_header pu_hdr;  // scratch header handed to generate_inter_prediction_samples, rewritten per PU
+  bool constrained_intra = false;  // rr_set_options
+  bool check_avail = false;
+  struct {  // first intra TU of the last rr_reconstruct whose record mask differs from the reference's own
+    bool found;
+    uint32_t tu;
+    uint64_t rec, ref;
+  } mismatch = {};
 
   const de265_image* get_image(uint16_t id) const override { return id < B200_MAX_SLOTS ? slot[id] : nullptr; }
   bool has_image(uint16_t id) const override { return id < B200_MAX_SLOTS && slot[id] != nullptr; }
@@ -133,6 +140,26 @@ int ensure_slot(Replay* r, int s, const b200_pic_params& p, const std::shared_pt
   return B200_OK;
 }
 
+// The availability mask of an intra TU as the reference derives it (intra_border_computer::preproc + fill_from_image,
+// intrapred.h:436-633, from the image's slice / tile / z-scan metadata and, with constrained_intra_pred_flag, its
+// prediction modes), packed like b200_tu.avail.  The sample values it gathers are ignored.
+template <class pixel_t>
+uint64_t reference_avail_mask(const de265_image* img, int xB, int yB, int nT, int cIdx)
+{
+  pixel_t border_mem[4 * MAX_INTRA_PRED_BLOCK_SIZE + 1];
+  intra_border_computer<pixel_t> c;
+  c.init(&border_mem[2 * MAX_INTRA_PRED_BLOCK_SIZE], img, nT, cIdx, xB, yB);
+  c.preproc();
+  c.fill_from_image();
+  uint64_t m = 0;
+  for (int k = 0; k < nT / 2; k++) {
+    if (c.available[-4 * k - 1]) m |= 1ull << k;
+    if (c.available[4 * k + 1]) m |= 1ull << (B200_AVAIL_TOP_BIT0 + k);
+  }
+  if (c.available[0]) m |= 1ull << B200_AVAIL_CORNER_BIT;
+  return m;
+}
+
 int tile_grid(const b200_picture* pic, int* cols, int* rows)
 {
   const b200_pic_params& p = pic->params;
@@ -159,6 +186,30 @@ EXPORT void* rr_create(int simd)
 }
 
 EXPORT void rr_destroy(void* h) { delete (Replay*)h; }
+
+// constrained_intra: replay with constrained_intra_pred_flag set, so the reference derives the availability of every intra
+// TU's neighbours from the prediction modes of the records (inter where a PU lies, intra where a luma intra / PCM TU lies).
+// check_avail: fail rr_reconstruct on the first intra TU whose record mask differs from the one the reference derives
+// (rr_avail_mismatch reports it).  Both are off after rr_create.
+EXPORT int rr_set_options(void* h, int constrained_intra, int check_avail)
+{
+  Replay* r = (Replay*)h;
+  if (!r) return B200_ERR_INVALID;
+  r->constrained_intra = constrained_intra != 0;
+  r->check_avail = check_avail != 0;
+  return B200_OK;
+}
+
+// 1 when the last rr_reconstruct stopped at an availability mismatch: the TU's index, the record's and the reference's masks.
+EXPORT int rr_avail_mismatch(void* h, uint32_t* tu, uint64_t* rec, uint64_t* ref)
+{
+  Replay* r = (Replay*)h;
+  if (!r || !r->mismatch.found) return 0;
+  *tu = r->mismatch.tu;
+  *rec = r->mismatch.rec;
+  *ref = r->mismatch.ref;
+  return 1;
+}
 
 EXPORT int rr_fill_slot(void* h, int s, const b200_pic_params* p, int vy, int vc)
 {
@@ -225,6 +276,8 @@ EXPORT int rr_reconstruct(void* h, const b200_picture* pic)
   de265_image* img = r->slot[p.dst_slot];
   seq_parameter_set* sps = hd.sps.get();
   pic_parameter_set* pps = hd.pps.get();
+  pps->constrained_intra_pred_flag = r->constrained_intra;
+  r->mismatch.found = false;
   img->set_headers(nullptr, hd.sps, hd.pps);
   img->clear_metadata();
   img->integrity = INTEGRITY_CORRECT;
@@ -317,6 +370,22 @@ EXPORT int rr_reconstruct(void* h, const b200_picture* pic)
   t->img = img;
   t->ResScaleVal = 0;
   t->explicit_rdpcm_flag = 0;
+  if (r->constrained_intra) {
+    // The prediction mode of every 8x8 block, as read_coding_unit would have stored it: CUs are at least 8x8 and 8-aligned, so
+    // each 8x8 belongs to one CU, inter where a PU lies, intra where a luma intra or PCM TU lies.
+    for (uint32_t i = 0; i < pic->n_pu; i++) {
+      const b200_pu& pu = pic->pus[i];
+      for (int y = pu.y & ~7; y < pu.y + pu.h; y += 8)
+        for (int x = pu.x & ~7; x < pu.x + pu.w; x += 8) img->set_pred_mode(x, y, 3, MODE_INTER);
+    }
+    for (uint32_t i = 0; i < pic->n_tu; i++) {
+      const b200_tu& tu = pic->tus[i];
+      if (tu.cidx || !(tu.flags & (B200_TU_INTRA | B200_TU_PCM))) continue;
+      const int nT = 1 << tu.log2_size;
+      for (int y = tu.y & ~7; y < tu.y + nT; y += 8)
+        for (int x = tu.x & ~7; x < tu.x + nT; x += 8) img->set_pred_mode(x, y, 3, MODE_INTRA);
+    }
+  }
   for (uint32_t i = 0; i < pic->n_tu; i++) {
     const b200_tu& tu = pic->tus[i];
     const int nT = 1 << tu.log2_size, c = tu.cidx;
@@ -335,6 +404,14 @@ EXPORT int rr_reconstruct(void* h, const b200_picture* pic)
     }
     const int xl = tu.x << (c ? 1 : 0), yl = tu.y << (c ? 1 : 0);  // luma position of the TU (4:2:0)
     if (tu.flags & B200_TU_INTRA) {
+      if (r->check_avail) {
+        const uint64_t ref = img->high_bit_depth(c) ? reference_avail_mask<uint16_t>(img, tu.x, tu.y, nT, c)
+                                                    : reference_avail_mask<uint8_t>(img, tu.x, tu.y, nT, c);
+        if (ref != tu.avail) {
+          r->mismatch = {true, i, tu.avail, ref};
+          return B200_ERR_INVALID;
+        }
+      }
       // disableIntraBoundaryFilter = implicit_rdpcm_enabled_flag && cu_transquant_bypass at (xB0, yB0) (intrapred.cc:308-310)
       const bool nbf = tu.flags & B200_TU_NO_BOUNDARY_FILTER;
       sps->range_extension.implicit_rdpcm_enabled_flag = nbf;
@@ -346,7 +423,9 @@ EXPORT int rr_reconstruct(void* h, const b200_picture* pic)
     }
     if (!(tu.flags & B200_TU_CBF)) continue;
     // scale_coefficients reads the CU's prediction mode at (xT, yT) for the DST / rotation decisions (transform.cc:400-404,
-    // 601-606) and the scaling-list matrix from its `intra` argument: make them say what the record says
+    // 601-606) and the scaling-list matrix from its `intra` argument: make them say what the record says.  (At component
+    // coordinates for chroma: with constrained_intra the 8x8's own mode is put back afterwards, later TUs read it.)
+    const PredMode cu_mode = img->get_pred_mode(tu.x & ~7, tu.y & ~7);
     img->set_pred_mode(tu.x & ~7, tu.y & ~7, 3, (tu.flags & (B200_TU_DST | B200_TU_ROTATE)) ? MODE_INTRA : MODE_INTER);
     sps->range_extension.transform_skip_rotation_enabled_flag = (tu.flags & B200_TU_ROTATE) != 0;
     t->cu_transquant_bypass_flag = (tu.flags & B200_TU_BYPASS) != 0;
@@ -359,6 +438,7 @@ EXPORT int rr_reconstruct(void* h, const b200_picture* pic)
     const bool matrix_intra = (tu.flags & B200_TU_SCALING_LIST) ? !(tu.flags & B200_TU_INTER_MATRIX) : (tu.flags & B200_TU_INTRA) != 0;
     const int rdpcm = (tu.flags & B200_TU_RDPCM_H) ? 1 : (tu.flags & B200_TU_RDPCM_V) ? 2 : 0;
     scale_coefficients(t, tu.x, tu.y, tu.x, tu.y, nT, c, (tu.flags & B200_TU_TSKIP) != 0, matrix_intra, rdpcm);
+    if (r->constrained_intra) img->set_pred_mode(tu.x & ~7, tu.y & ~7, 3, cu_mode);
     (void)xl; (void)yl;
   }
   sps->range_extension.transform_skip_rotation_enabled_flag = 0;

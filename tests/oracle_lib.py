@@ -100,15 +100,28 @@ def ref_replay_lib():
         lib.rr_fill_slot.argtypes = [vp, C.c_int, C.POINTER(capi.PicParams), C.c_int, C.c_int]
         lib.rr_upload_slot.argtypes = [vp, C.c_int, C.POINTER(capi.PicParams), capi.PlaneArray, capi.StrideArray]
         lib.rr_read_slot.argtypes = [vp, C.c_int, capi.PlaneArray, capi.StrideArray]
+        if hasattr(lib, "rr_set_options"):  # absent from a library built from an older oracle/ref_replay.cc
+            lib.rr_set_options.argtypes = [vp, C.c_int, C.c_int]
+            lib.rr_avail_mismatch.argtypes = [vp, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
         _rr = lib
     return _rr
 
 
+def ref_replay_has_options():
+    """True when the replay library takes the constrained_intra / check_avail options (rr_set_options).  A library shipped
+    prebuilt from an older oracle/ref_replay.cc lacks them: tests that need them then rely on the stored digests or skip."""
+    lib = ref_replay_lib()
+    return lib is not None and hasattr(lib, "rr_set_options")
+
+
 class RefReplay(Oracle):
     """Same interface as Oracle, executed by the reference's own code (simd=True: the table de265_acceleration_AUTO selects,
-    i.e. SSE4.1 + AVX2 + AVX-512 where the host has them; False: the scalar fallback table)."""
+    i.e. SSE4.1 + AVX2 + AVX-512 where the host has them; False: the scalar fallback table).
+    constrained_intra: the reference derives intra availability with constrained_intra_pred_flag set, from the records'
+    prediction modes.  check_avail: reconstruct() raises AvailMismatch at the first intra TU whose record mask differs from
+    the mask the reference derives."""
 
-    def __init__(self, simd=True):
+    def __init__(self, simd=True, constrained_intra=False, check_avail=False):
         lib = ref_replay_lib()
         if lib is None:
             raise RuntimeError("oracle/_ref/libref_replay.so not built (make -C oracle ref; needs /root/reference)")
@@ -116,5 +129,25 @@ class RefReplay(Oracle):
         class _Shim:  # present the rr_* entry points under the orc_* names the base class calls
             orc_destroy, orc_reconstruct, orc_upload_slot, orc_fill_slot, orc_read_slot = (lib.rr_destroy, lib.rr_reconstruct, lib.rr_upload_slot,
                                                                                            lib.rr_fill_slot, lib.rr_read_slot)
-        self.lib = _Shim
+        self.lib, self.rr = _Shim, lib
+        self.options = ref_replay_has_options()
+        if (constrained_intra or check_avail) and not self.options:
+            raise RuntimeError(f"{REPLAY_SO} predates rr_set_options: rebuild it (make -C oracle ref; needs /root/reference)")
         self.ctx = lib.rr_create(1 if simd else 0)
+        if self.options:
+            assert lib.rr_set_options(self.ctx, int(constrained_intra), int(check_avail)) == 0
+
+    def reconstruct(self, pic):
+        cp = getattr(pic, "c", pic)
+        rc = self.rr.rr_reconstruct(self.ctx, C.byref(cp))
+        i, rec, ref = C.c_uint32(), C.c_uint64(), C.c_uint64()
+        if self.options and self.rr.rr_avail_mismatch(self.ctx, C.byref(i), C.byref(rec), C.byref(ref)):
+            t = cp.tus[i.value]
+            raise AvailMismatch(f"TU {i.value} (x={t.x}, y={t.y}, {1 << t.log2_size}x{1 << t.log2_size}, cidx {t.cidx}): record avail "
+                                f"{rec.value:#x} != reference {ref.value:#x}")
+        if rc:
+            raise RuntimeError(f"rr_reconstruct failed: {rc}")
+
+
+class AvailMismatch(AssertionError):
+    """An intra TU's record availability mask differs from the one the reference derives."""

@@ -1,7 +1,8 @@
 """The edges of what a picture record may carry, as one shared case list: 4:0:0, 9 / 11 / 12 bit and unequal luma / chroma
 depths, QP' from 0 to 51 + QpBdOffset, deblocking and chroma QP offsets at +-12, explicit weights and offsets at the ends of
 their range, MVs anywhere in int16, SAO offsets at the legal maximum, the intra-smoothing / boundary-filter / PCM / per-slice
-filter switches.  test_cpu_range_edges.py pins the oracle to the reference on every case and test_gpu_range_edges.py the
+filter switches, intra availability masks with gaps (constrained intra prediction in P / B pictures, many slices).
+test_cpu_range_edges.py pins the oracle to the reference on every case and test_gpu_range_edges.py the
 engine to the oracle.
 
 Every case carries the checks that prove its edge is present in the generated records, so that the list cannot quietly turn
@@ -15,14 +16,71 @@ from libde265_b200 import capi, synth
 Case = namedtuple("Case", "id W H bd kw checks")
 
 
-def make_sequence(W, H, bd, **kw):
-    """Reference planes (uploaded to slot 5) and the I -> P -> B -> weighted B pictures of the parity tests' sequence."""
+def make_sequence(W, H, bd, pb_intra_frac=None, **kw):
+    """Reference planes (uploaded to slot 5) and the I -> P -> B -> weighted B pictures of the parity tests' sequence.
+    ``pb_intra_frac``: intra_frac of the P / B pictures (the I picture stays all intra)."""
     planes = synth.random_planes(W, H, bd, 99, bit_depth_chroma=kw.get("bit_depth_chroma"), chroma_format_idc=kw.get("chroma_format_idc", 1))
+    pb = {} if pb_intra_frac is None else dict(intra_frac=pb_intra_frac)
     pics = [synth.make_picture(W, H, "I", seed=11, dst_slot=0, bit_depth=bd, **kw),
-            synth.make_picture(W, H, "P", seed=12, dst_slot=1, ref_slots=(0, 5), bit_depth=bd, **kw),
-            synth.make_picture(W, H, "B", seed=13, dst_slot=2, ref_slots=(0, 1, 5), bit_depth=bd, **kw),
-            synth.make_picture(W, H, "B", seed=14, dst_slot=3, ref_slots=(0, 1, 2), weighted=True, bit_depth=bd, **kw)]
+            synth.make_picture(W, H, "P", seed=12, dst_slot=1, ref_slots=(0, 5), bit_depth=bd, **pb, **kw),
+            synth.make_picture(W, H, "B", seed=13, dst_slot=2, ref_slots=(0, 1, 5), bit_depth=bd, **pb, **kw),
+            synth.make_picture(W, H, "B", seed=14, dst_slot=3, ref_slots=(0, 1, 2), weighted=True, bit_depth=bd, **pb, **kw)]
     return planes, pics
+
+
+# ---- gaps in intra availability masks (b200_tu.avail: left groups from bit 0 down the column, corner bit 16, top groups from
+# bit 17 along the row; q = nT / 4 groups per side belong to the TU's own column / row, the next q to its bottom-left /
+# top-right reach) ----
+GAP_CLASSES = ("own_partial", "corner_missing", "reach_gap", "outer_only", "corner_only", "none_off_origin")
+SIZE_KINDS = ("4", "8y", "8c", "16", "32")
+
+
+def gap_class_counts(tus):
+    """{(class, size kind): number of intra TUs} over the TU records.  Classes: a partly available own column or row; own
+    column and row available but the corner missing; a reach that is not available up to a point from the inner end (so the
+    substitution is no clamp); own row missing with the top-right reach present, or own column missing with the bottom-left
+    present; only the corner; nothing available away from the picture origin.  Extra keys: ("8_top3_only", kind), an 8x8 TU
+    whose only available group is top group 3 (the 33rd border sample rides in its own register on the GPU), and
+    ("32_carry", "32"), a 32x32 TU that is no clamp and misses a sample at the start of a 32-sample scan chunk (s = 32, 64,
+    96, 128) while an earlier sample is available, so the chunk starts from the carried value."""
+    out = {}
+    for tu in tus[(tus["flags"] & capi.TU_INTRA) != 0]:
+        kind = {2: "4", 3: "8c" if tu["cidx"] else "8y", 4: "16", 5: "32"}[int(tu["log2_size"])]
+        for c in tu_gap_classes(tu):
+            out[(c, kind)] = out.get((c, kind), 0) + 1
+    return out
+
+
+def tu_gap_classes(tu):
+    """The gap classes of one intra TU record (see gap_class_counts)."""
+    log2, av = int(tu["log2_size"]), int(tu["avail"])
+    nT, q = 1 << log2, 1 << (log2 - 2)
+    g = (1 << q) - 1
+    lo, bl, co = av & g, (av >> q) & g, (av >> capi.AVAIL_CORNER_BIT) & 1
+    to, tr = (av >> capi.AVAIL_TOP_BIT0) & g, (av >> (capi.AVAIL_TOP_BIT0 + q)) & g
+    cls = []
+    if 0 < lo < g or 0 < to < g:
+        cls.append("own_partial")
+    if lo == g and to == g and not co:
+        cls.append("corner_missing")
+    if (bl & (bl + 1)) or (tr & (tr + 1)):
+        cls.append("reach_gap")
+    if (to == 0 and tr) or (lo == 0 and bl):
+        cls.append("outer_only")
+    if av == 1 << capi.AVAIL_CORNER_BIT:
+        cls.append("corner_only")
+    if av == 0 and (tu["x"], tu["y"]) != (0, 0):
+        cls.append("none_off_origin")
+    if nT == 8 and av == 1 << (capi.AVAIL_TOP_BIT0 + 3):
+        cls.append("8_top3_only")
+    if nT == 32 and not (lo == g and to == g and co and "reach_gap" not in cls):
+        # scan sample s -> availability; chunk starts s = 32 (left row 31), 64 (corner), 96 (top column 31), 128 (top column 63)
+        def avail_at(s):
+            i = s - 64
+            return (av >> ((-i - 1) >> 2)) & 1 if i < 0 else co if i == 0 else (av >> (capi.AVAIL_TOP_BIT0 + ((i - 1) >> 2))) & 1
+        if any(not avail_at(s) and any(avail_at(e) for e in range(s)) for s in (32, 64, 96, 128)):
+            cls.append("32_carry")
+    return cls
 
 
 # ---- checks: (description, predicate over the sequence's pictures) ----
@@ -164,6 +222,49 @@ def bs_zero_in_disabled_slices():
     return "slices with deblocking off have bS 0 on their edges", f
 
 
+GEOMETRY_FORBIDS = {("own_partial", "4"), ("own_partial", "8y"), ("reach_gap", "4"), ("reach_gap", "8y")}  # one 8x8 CU per 8 luma samples
+
+
+def gap_counts(pics):
+    cnt = {}
+    for p in pics:
+        for k, v in gap_class_counts(p.tus).items():
+            cnt[k] = cnt.get(k, 0) + v
+    return cnt
+
+
+def gaps(kinds=SIZE_KINDS, classes=GAP_CLASSES, skip=()):
+    """Every gap class at every TU size kind, except where the geometry rules it out (a 4x4 / 8x8 luma TU's own column, own
+    row and reach each lie in one 8x8 CU) and the listed (class, kind) pairs that the case's sizes make rare."""
+    want = [(c, k) for c in classes for k in kinds if (c, k) not in GEOMETRY_FORBIDS and (c, k) not in skip]
+
+    def f(pics):
+        cnt = gap_counts(pics)
+        return all(cnt.get(w, 0) > 0 for w in want)
+    return f"intra TUs with availability gaps of each class {want}", f
+
+
+def top3_only():
+    return "an 8x8 TU whose only available group is top group 3", lambda pics: any(k[0] == "8_top3_only" for k in gap_counts(pics))
+
+
+def carry32():
+    return "a 32x32 TU whose substitution carries a value into a 32-sample chunk", lambda pics: gap_counts(pics).get(("32_carry", "32"), 0) > 0
+
+
+def smoothed_32_on_substituted_border(n):
+    def f(pics):
+        t = _tus(pics)
+        t = t[((t["flags"] & capi.TU_INTRA) != 0) & (t["log2_size"] == 5) & (t["cidx"] == 0)]
+        g = np.uint64(0xFF)
+        av = t["avail"].astype(np.uint64)
+        own = ((av & g) == g) & (((av >> np.uint64(capi.AVAIL_CORNER_BIT)) & np.uint64(1)) == 1) & (((av >> np.uint64(capi.AVAIL_TOP_BIT0)) & g) == g)
+        m = t["intra_mode"].astype(np.int64)
+        smoothed = (m != 1) & (np.minimum(np.abs(m - 26), np.abs(m - 10)) > 0)
+        return int((~own & smoothed).sum()) >= n
+    return f"{n} 32x32 luma TUs with a smoothed mode and a gap in their own column, corner or row", f
+
+
 def ctb_grid(log2, W, H):
     return f"CTB {1 << log2} on a {W}x{H} picture", lambda pics: all(p.params.log2_ctb_size == log2 and (p.params.width, p.params.height) == (W, H)
                                                                      for p in pics)
@@ -171,6 +272,7 @@ def ctb_grid(log2, W, H):
 
 # ---- the case list: (id, W, H, bd, make_picture kwargs, checks) ----
 _PCM = dict(special_frac=0.12, cbf_prob=0.9)
+_CIP = dict(constrained_intra=True, pb_intra_frac=0.5)
 
 CASES = [
     Case("mono8_ctb64", 192, 128, 8, dict(chroma_format_idc=0, **_PCM), [no_chroma_tus(), ctb_grid(6, 192, 128), tu_flag(capi.TU_PCM, "PCM")]),
@@ -214,7 +316,29 @@ CASES = [
     Case("mono8_tiles_slice_flags", 448, 256, 8, dict(chroma_format_idc=0, tiles=(2, 3), n_slices=5, slice_deblock_off_frac=0.4, slice_sao_off_frac=0.5),
          [no_chroma_tus(), slice_flag_mix(capi.SLICE_SAO_LUMA, "SAO luma"), bs_zero_in_disabled_slices()]),
     Case("skip_sao10", 192, 128, 10, dict(skip_sao=True, sao_offset="max"), [pic_flag(capi.PIC_SKIP_SAO, True, "SKIP_SAO")]),
+    # Constrained intra prediction: half the CUs of the P / B pictures are intra, and their inter neighbours are unavailable, so
+    # gaps fall anywhere in the border (own column, corner, own row, either reach).  The last case is the source of gaps without
+    # it: slice boundaries between the CTB above and the one above-right / above-left.
+    Case("cip8_ctb64", 448, 256, 8, dict(size_area=(0.0, 0.5, 0.25, 0.25), **_CIP),
+         [gaps(skip=(("corner_missing", "32"), ("corner_only", "32"))), top3_only(), carry32()]),
+    Case("cip8_ctb32_small_cus", 320, 192, 8, dict(log2_ctb=5, size_area=(0.0, 0.2, 0.4, 0.4), **_CIP),
+         [gaps(skip=(("corner_missing", "32"), ("corner_only", "32"))), top3_only(), carry32()]),
+    Case("cip8_ctb16", 208, 120, 8, dict(log2_ctb=4, size_area=(0.0, 0.0, 0.5, 0.5), **_CIP),
+         [ctb_grid(4, 208, 120), gaps(kinds=("4", "8y", "8c", "16"), skip=(("corner_only", "8c"), ("corner_only", "16")))]),
+    Case("cip10_tiles_slices", 448, 256, 10, dict(tiles=(3, 2), lf_across_tiles=False, n_slices=5, size_area=(0.0, 0.4, 0.3, 0.3), **_CIP),
+         [gaps(skip=(("corner_missing", "32"), ("corner_only", "32"))), top3_only(), carry32()]),
+    Case("cip12_chroma9", 320, 192, 12, dict(bit_depth_chroma=9, size_area=(0.0, 0.4, 0.3, 0.3), **_CIP),
+         [gaps(skip=(("corner_missing", "32"), ("corner_only", "8c"), ("corner_only", "16"), ("corner_only", "32"))), carry32()]),
+    Case("cip_mono8", 320, 192, 8, dict(chroma_format_idc=0, size_area=(0.0, 0.5, 0.25, 0.25), **_CIP),
+         [no_chroma_tus(), gaps(kinds=("4", "8y", "16", "32"), skip=(("corner_missing", "32"), ("corner_only", "32"))), carry32()]),
+    Case("cip8_smoothing_off", 320, 192, 8, dict(intra_smoothing_off=True, size_area=(0.0, 0.5, 0.25, 0.25), **_CIP),
+         [pic_flag(capi.PIC_INTRA_SMOOTHING_OFF, True, "INTRA_SMOOTHING_OFF"), gaps(skip=(("corner_missing", "32"),)), top3_only(), carry32()]),
+    Case("cip8_strong_smoothing", 448, 256, 8, dict(size_area=(0.3, 0.5, 0.1, 0.1), **_CIP),
+         [pic_flag(capi.PIC_STRONG_INTRA_SMOOTHING, True, "STRONG_INTRA_SMOOTHING"), gaps(), carry32(), smoothed_32_on_substituted_border(20)]),
+    Case("intra8_24_slices", 416, 240, 8, dict(log2_ctb=5, n_slices=24, pb_intra_frac=1.0),
+         [gaps(classes=("corner_missing", "outer_only", "none_off_origin"), skip=(("corner_missing", "8c"), ("outer_only", "32"))), carry32()]),
 ]
+CIP_CASE_IDS = [c.id for c in CASES if c.kw.get("constrained_intra")]
 
 CASE_IDS = [c.id for c in CASES]
 BY_ID = {c.id: c for c in CASES}

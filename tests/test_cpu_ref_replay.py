@@ -54,6 +54,19 @@ def run_sequence(pins, W, H, bd, simd, log2_ctb=6, stages=True, **kw):
         ref.close()
 
 
+# The sequences the tests below replay, as (W, H, bit depth, run_sequence keywords); test_cpu_range_edges.py also checks their
+# availability masks against the reference.
+EVERY_STAGE = [(416, 240, bd, {}) for bd in (8, 10)]
+RAGGED = [(8, 8, 8, {}), (72, 40, 8, {}), (200, 136, 8, {}), (1288, 8, 8, {}),
+          (208, 120, 8, dict(log2_ctb=4, size_area=(0.0, 0.0, 0.5, 0.5))), (208, 120, 10, dict(log2_ctb=5, size_area=(0.0, 0.3, 0.4, 0.3)))]
+SPECIAL = [(320, 192, 8, dict(n_slices=4, scaling_list=True)),
+           (320, 192, 10, dict(deblock=False, sao=False, stages=False)),
+           (320, 192, 8, dict(special_frac=0.15, cbf_prob=0.9)),
+           (320, 192, 10, dict(special_frac=0.2, cbf_prob=0.9, rdpcm_frac=0.5, rotate_frac=0.5, tskip_max_log2=5)),
+           (448, 256, 8, dict(tiles=(3, 2), lf_across_tiles=False)),
+           (448, 256, 10, dict(tiles=(2, 3), lf_across_tiles=True, n_slices=3))]
+
+
 @pytest.mark.parametrize("simd", [False, True])
 @pytest.mark.parametrize("bd", [8, 10])
 def test_replay_matches_oracle_every_stage(pins, bd, simd):
@@ -62,20 +75,14 @@ def test_replay_matches_oracle_every_stage(pins, bd, simd):
 
 @pytest.mark.parametrize("simd", [False, True])
 def test_replay_ragged_sizes_and_small_ctbs(pins, simd):
-    for size in ((8, 8), (72, 40), (200, 136), (1288, 8)):
-        run_sequence(pins, size[0], size[1], 8, simd, stages=False)
-    run_sequence(pins, 208, 120, 8, simd, log2_ctb=4, stages=False, size_area=(0.0, 0.0, 0.5, 0.5))
-    run_sequence(pins, 208, 120, 10, simd, log2_ctb=5, stages=False, size_area=(0.0, 0.3, 0.4, 0.3))
+    for W, H, bd, kw in RAGGED:
+        run_sequence(pins, W, H, bd, simd, stages=False, **kw)
 
 
 @pytest.mark.parametrize("simd", [False, True])
 def test_replay_slices_scaling_lists_special_blocks_tiles(pins, simd):
-    run_sequence(pins, 320, 192, 8, simd, n_slices=4, scaling_list=True)
-    run_sequence(pins, 320, 192, 10, simd, deblock=False, sao=False, stages=False)
-    run_sequence(pins, 320, 192, 8, simd, special_frac=0.15, cbf_prob=0.9)
-    run_sequence(pins, 320, 192, 10, simd, special_frac=0.2, cbf_prob=0.9, rdpcm_frac=0.5, rotate_frac=0.5, tskip_max_log2=5)
-    run_sequence(pins, 448, 256, 8, simd, tiles=(3, 2), lf_across_tiles=False)
-    run_sequence(pins, 448, 256, 10, simd, tiles=(2, 3), lf_across_tiles=True, n_slices=3)
+    for W, H, bd, kw in SPECIAL:
+        run_sequence(pins, W, H, bd, simd, **kw)
 
 
 def test_replay_missing_reference_and_fill(pins):
