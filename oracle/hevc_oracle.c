@@ -707,11 +707,10 @@ static int surf_ensure(orc_surface* s, const b200_pic_params* p)
 {
   const pic_geom g = geom_of(p);
   int cw = p->chroma_format_idc ? p->width / g.sub_w : 0, ch = p->chroma_format_idc ? p->height / g.sub_h : 0;
-  if (s->plane[0] && s->width == p->width && s->height == p->height && s->chroma_format_idc == p->chroma_format_idc) {
-    s->bd_y = p->bit_depth_luma;
-    s->bd_c = p->bit_depth_chroma;
+  /* any format difference starts a new zero-filled picture, as the reference's image allocation does (ref_replay.cc ensure_slot) */
+  if (s->plane[0] && s->width == p->width && s->height == p->height && s->chroma_format_idc == p->chroma_format_idc &&
+      s->bd_y == p->bit_depth_luma && s->bd_c == p->bit_depth_chroma)
     return 0;
-  }
   surf_free(s);
   s->width = p->width; s->height = p->height; s->cw = cw; s->ch = ch;
   s->chroma_format_idc = p->chroma_format_idc;
@@ -795,6 +794,10 @@ static void inter_pred_pu(orc_ctx* c, orc_surface* cur, const b200_picture* pic,
   for (int l = 0; l < 2; l++) {
     if (!use[l]) continue;
     const orc_surface* ref = pu->ref_slot[l] >= 0 ? orc_slot(c, pu->ref_slot[l]) : NULL;
+    /* motion.cc:385-405: a reference of another size, chroma format or luma / chroma bit depth counts as missing */
+    if (ref && (ref->width != pic->params.width || ref->height != pic->params.height || ref->chroma_format_idc != pic->params.chroma_format_idc ||
+                ref->bd_y != pic->params.bit_depth_luma || ref->bd_c != pic->params.bit_depth_chroma))
+      ref = NULL;
     if (!ref) { /* motion.cc:362-376: mid-grey in 14-bit intermediate precision */
       for (int k = 0; k < nc; k++)
         for (int i = 0; i < 64 * 64; i++) pred[l][k][i] = 1 << 13;

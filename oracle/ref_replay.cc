@@ -120,22 +120,30 @@ de265_chroma chroma_of(int idc)
   return idc == 0 ? de265_chroma_mono : idc == 1 ? de265_chroma_420 : idc == 2 ? de265_chroma_422 : de265_chroma_444;
 }
 
-// (Re)allocates the slot's image when the geometry changed; the samples of an existing image are kept.
+// (Re)allocates the slot's image when the format changed; the samples of an existing image are kept.  A new CTB size alone
+// keeps the samples too, but needs a new image: the per-CTB metadata is allocated for the CTB grid of the image's first SPS.
 int ensure_slot(Replay* r, int s, const b200_pic_params& p, const std::shared_ptr<seq_parameter_set>& sps)
 {
   de265_image*& img = r->slot[s];
-  if (img && img->get_width(0) == p.width && img->get_height(0) == p.height && img->get_chroma_format() == chroma_of(p.chroma_format_idc) &&
-      img->get_bit_depth(0) == p.bit_depth_luma && img->get_bit_depth(1) == p.bit_depth_chroma) {
-    return B200_OK;
-  }
-  delete img;
-  img = new de265_image();
-  if (img->alloc_image(p.width, p.height, chroma_of(p.chroma_format_idc), sps, true, &r->dctx, 0, nullptr, false) != DE265_OK) {
-    delete img;
-    img = nullptr;
+  const bool same_format = img && img->get_width(0) == p.width && img->get_height(0) == p.height &&
+                           img->get_chroma_format() == chroma_of(p.chroma_format_idc) && img->get_bit_depth(0) == p.bit_depth_luma &&
+                           img->get_bit_depth(1) == p.bit_depth_chroma;
+  if (same_format && img->number_of_ctbs() == (uint32_t)sps->PicSizeInCtbsY) return B200_OK;
+  de265_image* fresh = new de265_image();
+  if (fresh->alloc_image(p.width, p.height, chroma_of(p.chroma_format_idc), sps, true, &r->dctx, 0, nullptr, false) != DE265_OK) {
+    delete fresh;
     return B200_ERR_NOMEM;
   }
-  img->fill_image(0, 0, 0);  // new surfaces start at zero like the engine's and the oracle's
+  fresh->fill_image(0, 0, 0);  // new surfaces start at zero like the engine's and the oracle's
+  if (same_format)
+    for (int c = 0; c < (p.chroma_format_idc ? 3 : 1); c++) {
+      const int bpp = img->get_bytes_per_pixel(c);
+      for (int y = 0; y < img->get_height(c); y++)
+        memcpy(fresh->get_image_plane(c) + (size_t)y * fresh->get_image_stride(c) * bpp,
+               img->get_image_plane(c) + (size_t)y * img->get_image_stride(c) * bpp, (size_t)img->get_width(c) * bpp);
+    }
+  delete img;
+  img = fresh;
   img->PicState = UsedForShortTermReference;
   return B200_OK;
 }
@@ -186,6 +194,10 @@ EXPORT void* rr_create(int simd)
 }
 
 EXPORT void rr_destroy(void* h) { delete (Replay*)h; }
+
+// Present from the version whose ensure_slot reallocates a slot's image on a CTB-size change.  A library built from an older
+// ref_replay.cc lacks it: it keeps the image, whose per-CTB metadata is then too small for a smaller CTB, and corrupts the heap.
+EXPORT int rr_handles_ctb_change(void) { return 1; }
 
 // constrained_intra: replay with constrained_intra_pred_flag set, so the reference derives the availability of every intra
 // TU's neighbours from the prediction modes of the records (inter where a PU lies, intra where a luma intra / PCM TU lies).

@@ -114,6 +114,14 @@ def ref_replay_has_options():
     return lib is not None and hasattr(lib, "rr_set_options")
 
 
+def ref_replay_handles_ctb_change():
+    """True when the replay library reallocates a slot's image on a CTB-size change (rr_handles_ctb_change).  A library shipped
+    prebuilt from an older oracle/ref_replay.cc corrupts its heap when a name is rewritten with a smaller CTB: tests that
+    need it then rely on the stored digests."""
+    lib = ref_replay_lib()
+    return lib is not None and hasattr(lib, "rr_handles_ctb_change")
+
+
 class RefReplay(Oracle):
     """Same interface as Oracle, executed by the reference's own code (simd=True: the table de265_acceleration_AUTO selects,
     i.e. SSE4.1 + AVX2 + AVX-512 where the host has them; False: the scalar fallback table).
