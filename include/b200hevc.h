@@ -304,11 +304,14 @@ B200_API void* b200_engine_stream(b200_engine*);
 /* ... after making stream 0 wait for everything issued so far on the other streams. */
 B200_API int  b200_engine_join(b200_engine*);
 
-/* Host-side planner without a device (diagnostics / tests of the host logic on machines without a GPU): validates the
- * records exactly as b200_engine_submit_picture does and returns the work lists the kernels would consume.
+/* Host-side planner without a device (diagnostics / tests of the host logic on machines without a GPU): runs the planning
+ * b200_engine_submit_picture runs, under the planner switches b200_engine_create reads (B200_REGION, B200_INTRA_ORDER,
+ * B200_INTRA_SPLIT, B200_MC_LEGACY), and returns the work lists the kernels would consume.
  * counts[8] = { n_mc_units, n_list_a, n_list_a_warp_class, n_list_a_8x8_class, n_list_b, n_tasks, ref_slot_mask, 0 }.
  * Each output array may be NULL; otherwise it must hold cap_* entries and receives min(count, cap) of them:
- *   mc_units   one word per <= 8x16 (8 bit) / <= 16x16 (> 8 bit) MC unit: bits 0-19 PU index, the rest the unit's position in the PU
+ *   mc_units   one word per MC unit, bits 0-19 the PU index, the rest the unit's position in the PU.  8 bit: <= 16x16 tiles tagged
+ *              with their class (bits 24-26), sorted into class-pure batches padded with 0xFFFFFFFF; > 8 bit: plain <= 16x16
+ *              tiles; with B200_MC_LEGACY=1 (8 bit): <= 8x16 units
  *   list_a     indices of the non-intra TUs with work: warp class | 8x8 class | 4x4 class
  *   list_b     indices of the intra TUs grouped by task, tasks in the order the intra kernel claims them (topological)
  *   task_start n_tasks + 1 offsets into list_b */

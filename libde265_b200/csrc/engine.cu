@@ -1,7 +1,7 @@
 // engine.cu — host side of the B200 reconstruction engine (b200hevc.h part 2) + kernel launches.
 //
 // Per picture: validate the records, build the work lists (MC units, k_residual classes, intra tasks in topological
-// order) and pack everything into one pinned staging buffer on a small host thread pool, ONE host->device copy, then
+// order) and pack everything into one pinned staging buffer on a small host thread pool (planner.cuh), ONE host->device copy, then
 //   k_inter_pred8 -> k_residual -> k_mark_pending + k_intra -> k_deblock<V> -> k_deblock<H> -> k_sao_prep + k_sao
 // on one of the engine's streams; pictures are pipelined over the streams with per-slot event ordering.
 // Reference pictures never leave the device (DPB slots are device surfaces).
@@ -15,6 +15,7 @@
 #include <deque>
 #include <exception>
 #include <functional>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <sched.h>
@@ -226,14 +227,13 @@ struct StagingSet {
 // A few host threads for the per-picture host work (validation / work-list building of the PUs next to that of the TUs,
 // copying the record arrays into the pinned staging buffer): submit_picture is host-bound on large pictures otherwise.
 struct HostPool {
-  // Jobs belong to a group; wait(group) returns when that group's jobs are done, so several threads (the asynchronous planners)
-  // can share one pool.
+  // Jobs belong to a group; wait(group) returns when that group's jobs are done, so several planners (the engine's and the
+  // asynchronous ones) can share one pool.
   struct Group { int pending = 0; };
   std::vector<std::thread> th;
   std::mutex m;
   std::condition_variable cv, done_cv;
   std::deque<std::pair<Group*, std::function<void()>>> q;
-  Group own;
   bool stop = false;
   void start(int n)
   {
@@ -271,8 +271,6 @@ struct HostPool {
     std::unique_lock<std::mutex> lk(m);
     done_cv.wait(lk, [g] { return g->pending == 0; });
   }
-  void run(std::function<void()> f) { run(&own, std::move(f)); }
-  void wait() { wait(&own); }
   ~HostPool()
   {
     {
@@ -283,6 +281,8 @@ struct HostPool {
     for (auto& t : th) t.join();
   }
 };
+
+#include "planner.cuh"
 
 // One pipeline context = one CUDA stream with everything a picture in flight needs privately.  Pictures are issued
 // round-robin onto the contexts; cross-context ordering comes from per-slot events (SlotSync): a picture waits for the
@@ -305,13 +305,6 @@ struct SlotSync {
   int writer = -1;                       // context of the last writer, -1: none in flight
   cudaEvent_t read[B200_MAX_CTX] = {};   // last read of this slot issued on each context
   bool read_pending[B200_MAX_CTX] = {};
-};
-
-#define PLAN_PU_PARTS 4
-#define PLAN_INTRA_PARTS 8
-struct IntraPart {
-  uint32_t i0 = 0, i1 = 0, task_base = 0;
-  std::vector<uint32_t> intra_idx, task_of, task_first, task_cell, diag_cnt, diag_off, fill;  // task_cell: region cell x | y << 12 | cells per side << 24 | plane << 28
 };
 
 struct AsyncState;
@@ -348,40 +341,21 @@ struct b200_engine {
     for (int& v : last_owner) v = -1;
   }
   HostPool pool;
-  // A shadow engine (asynchronous planner) plans a picture on its own thread; for a picture with a long plan (a large intra
-  // picture) it borrows the owning engine's pool so that the in-order sequencer is not held up by it.
-  HostPool* helper = nullptr;
-  HostPool::Group helper_group;
-  bool use_helper = false;
-  void prun(std::function<void()> f)
-  {
-    if (use_helper) helper->run(&helper_group, std::move(f));
-    else pool.run(std::move(f));
-  }
-  void pwait()
-  {
-    if (use_helper) helper->wait(&helper_group);
-    else pool.wait();
-  }
+  Planner planner;  // b200_engine_submit_picture / _prepare_picture, every picture on `pool`
   int num_sms = 132;
   long long slot_depth[B200_MAX_SLOTS] = {}, tail_depth[B200_MAX_CTX] = {}, key_depth = 0;  // pick_ctx: dependency depths
-  // one intra task per plane and region in every picture (default).  B200_INTRA_SPLIT=0: pictures with inter prediction merge the
-  // planes of a region into one task — fewer tasks, but each runs its segments in sequence (three dependent L2 round trips)
-  bool intra_split_planes = true;
   bool sched_rr = false;        // B200_SCHED=rr: plain round-robin placement (A/B measurements)
   int n_ind = 2, next_ind = 0, ind_run = 0;  // streams for pictures that read no reference (intra pictures), used round-robin (B200_IND_STREAMS)
   int intra_i_grid = 64;        // grid cap of k_intra for such pictures: the DAG is at most ~160 tasks wide, 64 CTAs (512 warps) cover it and leave the other SMs to the P/B pictures (0: one CTA per SM; B200_INTRA_I_GRID)
   unsigned int *intra_err = nullptr, *intra_err_host = nullptr;  // k_intra gave up a dependency wait (device word; mapped host copy)
   unsigned long long spin_limit_ns = 2000000000ull;              // B200_INTRA_SPIN_LIMIT_MS
   int intra_ctas = 3, poll_ns = 256;  // k_intra: persistent CTAs per SM, back-off cap of the flag polling (B200_INTRA_CTAS / B200_POLL_NS)
-  int region = 16;  // luma size of an intra region task (16 or 8; B200_REGION overrides)
   // B200_TIMELINE=<file>: a CUDA event before and after every launch; the intervals of all streams (ms since the first launch)
   // are appended to the file at b200_engine_sync / destroy: which kernels of which pictures really overlap (tools/timeline.py)
   struct TlEntry { cudaEvent_t e0, e1; const char* name; int poc, ctx; };
   std::vector<TlEntry> tl;
   const char* tl_path = nullptr;
   cudaEvent_t tl_base = nullptr;
-  bool mc_legacy = false;  // B200_MC_LEGACY=1: the first-generation 8-bit MC kernel (k_inter_pred8) for A/B measurements
   int mc_ctas = 3;         // k_inter_pred_tma: persistent CTAs per SM (B200_MC_CTAS)
   bool timing = false;
   std::vector<cudaEvent_t> tev;  // timing ring: TIMING_RING pictures x 7 events
@@ -396,15 +370,6 @@ struct b200_engine {
   uint64_t async_n = 0;
   bool host_prof = false;
   int host_skip = 0;
-  // host scratch reused across pictures
-  std::vector<uint32_t> part_a[8][3];  // plan_intra_A: per range, per k_residual class
-  std::vector<uint32_t> pu_tiles[PLAN_PU_PARTS];  // plan_pus_part
-  size_t pu_count[PLAN_PU_PARTS][8] = {};
-  uint32_t pu_ref_mask[PLAN_PU_PARTS] = {};
-  IntraPart ipart[PLAN_INTRA_PARTS];              // plan_intra_*
-  std::vector<uint32_t> cell_level[3], task_level, level_off;  // plan_intra_levels
-  int intra_level_order = 2;  // 2: every picture by DAG level, 1: intra pictures only (B200_INTRA_ORDER=level_i), 0: CTB anti-diagonal order everywhere (=diag)
-  std::vector<uint32_t> ctb_count, tiles, tiles_sorted, list_a, list_b, intra_idx, diag_count, task_of, task_first, task_start, task_order;
 };
 
 static int async_flush(b200_engine* en);
@@ -443,19 +408,6 @@ static void tl_flush(b200_engine* en)  // after all streams were synchronised
     launch;                                                                           \
     if (en->tl_path) tl_end(en, st);                                                  \
   } while (0)
-
-struct PicLayout {
-  size_t off[14] = {}, total = 0, raw_total = 0, unit_cap = 0;
-  uint32_t ref_mask = 0;  // slots the picture's PUs read
-  int n_tiles = 0, n_batches = 0, n_a = 0, n_aw = 0, n_a8 = 0, n_b = 0, n_task = 0;
-  bool direct = false;                   // B200_PIC_RECORDS_PINNED: raw sections are uploaded from raw_src (the caller's arrays)
-  const void* raw_src[14] = {};
-  size_t raw_sz[14] = {};
-  int intra_levels = 0, intra_width = 0;  // tickets in DAG-level order: number of levels, tasks in the widest level (0: anti-diagonal order)
-  bool run_deblock = false, run_sao = false, has_scaling = false;
-  b200_pic_params params{};
-  uint32_t n_tu = 0;
-};
 
 struct b200_prepared {
   uint8_t* dev = nullptr;
@@ -528,8 +480,9 @@ extern "C" int b200_engine_create(b200_engine** out, int device)
     if (const char* e = getenv("B200_HOST_THREADS")) nt = std::max(0, std::min(16, atoi(e)));
     en->pool.start(nt);
   }
+  en->planner.opt = plan_options_from_env();
+  en->planner.pool = &en->pool;
   if (const char* e = getenv("B200_INTRA_CTAS")) en->intra_ctas = std::max(1, std::min(4, atoi(e)));
-  if (const char* e = getenv("B200_INTRA_SPLIT")) en->intra_split_planes = atoi(e) != 0;
   if (const char* e = getenv("B200_SCHED")) en->sched_rr = !strcmp(e, "rr");
   if (const char* e = getenv("B200_IND_STREAMS")) en->n_ind = std::max(1, std::min(4, atoi(e)));
   if (const char* e = getenv("B200_INTRA_I_GRID")) en->intra_i_grid = std::max(0, atoi(e));
@@ -538,12 +491,9 @@ extern "C" int b200_engine_create(b200_engine** out, int device)
   if (const char* e = getenv("B200_SAO_LEGACY")) en->sao_legacy = atoi(e) != 0;
   if (const char* e = getenv("B200_POLL_NS")) en->poll_ns = std::max(32, std::min(100000, atoi(e)));
   if (const char* e = getenv("B200_INTRA_SPIN_LIMIT_MS")) en->spin_limit_ns = 1000000ull * (unsigned long long)std::max(1, std::min(60000, atoi(e)));
-  if (const char* e = getenv("B200_REGION")) en->region = (atoi(e) == 8) ? 8 : 16;
-  if (const char* e = getenv("B200_INTRA_ORDER")) en->intra_level_order = !strcmp(e, "diag") ? 0 : !strcmp(e, "level_i") ? 1 : 2;
   en->tl_path = getenv("B200_TIMELINE");
   en->host_prof = getenv("B200_HOST_PROF") != nullptr;
   if (const char* e = getenv("B200_HOST_PROF_SKIP")) en->host_skip = std::max(0, atoi(e));
-  if (const char* e = getenv("B200_MC_LEGACY")) en->mc_legacy = atoi(e) != 0;
   if (const char* e = getenv("B200_MC_CTAS")) en->mc_ctas = std::max(1, std::min(8, atoi(e)));
   if (const char* e = getenv("B200_STREAMS")) en->n_ctx = std::max(1, std::min(B200_MAX_CTX, atoi(e)));
   for (int k = 0; k < B200_MAX_CTX; k++) {
@@ -717,19 +667,6 @@ extern "C" int b200_engine_timing_sum(b200_engine* en, float ms[6], int* n_pictu
   return B200_OK;
 }
 
-static int check_params(const b200_pic_params& p)
-{
-  if (p.width == 0 || p.height == 0) return set_err(B200_ERR_INVALID, "empty picture");
-  if (p.log2_ctb_size < 4 || p.log2_ctb_size > 6) return set_err(B200_ERR_INVALID, "log2_ctb_size %d", p.log2_ctb_size);
-  if (p.dst_slot >= B200_MAX_SLOTS) return set_err(B200_ERR_INVALID, "dst_slot %d", p.dst_slot);
-  if (p.chroma_format_idc > 1) return set_err(B200_ERR_UNSUPPORTED, "chroma_format_idc %d: the device path implements 4:0:0 and 4:2:0", p.chroma_format_idc);
-  if (p.bit_depth_luma < 8 || p.bit_depth_luma > 12 || p.bit_depth_chroma < 8 || p.bit_depth_chroma > 12)
-    return set_err(B200_ERR_UNSUPPORTED, "bit depth %d/%d (8..12 supported)", p.bit_depth_luma, p.bit_depth_chroma);
-  if ((p.bit_depth_luma > 8) != (p.bit_depth_chroma > 8)) return set_err(B200_ERR_UNSUPPORTED, "mixed 8-bit / high-bit-depth planes");
-  if ((p.width & 7) || (p.height & 7)) return set_err(B200_ERR_INVALID, "picture size must be a multiple of the minimum CB size (8)");
-  return B200_OK;
-}
-
 static DevPic make_devpic(const b200_pic_params& p, const Surface& cur, const Surface& out)
 {
   DevPic d{};
@@ -764,7 +701,7 @@ static int launch_picture(b200_engine* en, PipeCtx& cx, const PicLayout& L, cons
   const bool run_deblock = L.run_deblock, run_sao = L.run_sao;
   if (en->timing) CU(cudaEventRecord(en->ev[1], st));
   if (n_tiles > 0) {
-    if (sizeof(P) == 1 && !en->mc_legacy) {
+    if (L.mc_units == MC_CLASS_BATCHES) {
       // reference windows staged by TMA: the tensor maps of the slots this picture reads travel as a kernel parameter
       MctMaps maps;
       memset(&maps, 0, sizeof(maps));
@@ -780,7 +717,7 @@ static int launch_picture(b200_engine* en, PipeCtx& cx, const PicLayout& L, cons
       const uint32_t* tw = (const uint32_t*)(dbase + off[12]);  // tile words, then the batch table
       TL("mc", (k_inter_pred_tma<<<std::min(L.n_batches, en->num_sms * en->mc_ctas), MCT_CTA_THREADS, sizeof(MctShared), st>>>(
                    dp, maps, (const b200_pu*)(dbase + off[0]), (const b200_weight_entry*)(dbase + off[1]), tw, tw + n_tiles, L.n_batches)));
-    } else if (sizeof(P) == 1)
+    } else if (L.mc_units == MC_UNITS8x16)
       k_inter_pred8<<<std::min((n_tiles + MC8_UNITS_PER_CTA - 1) / MC8_UNITS_PER_CTA, en->num_sms * 5), MC8_WARPS * 32, 0, st>>>(dp, refs, (const b200_pu*)(dbase + off[0]), (const b200_weight_entry*)(dbase + off[1]),
                                                          (const uint32_t*)(dbase + off[12]), n_tiles);
     else
@@ -795,7 +732,7 @@ static int launch_picture(b200_engine* en, PipeCtx& cx, const PicLayout& L, cons
     ra.coeffs = (const b200_coeff*)(dbase + off[5]);
     ra.scaling = L.has_scaling ? dbase + off[11] : nullptr;
     ra.ticket = (unsigned int*)cx.sync_buf;
-    ra.region = en->region;
+    ra.region = L.region;
     ra.poll_ns = en->poll_ns;
     ra.err = en->intra_err;
     ra.err_host = en->intra_err_host;
@@ -912,490 +849,6 @@ static int launch_picture(b200_engine* en, PipeCtx& cx, const PicLayout& L, cons
   return B200_OK;
 }
 
-// Validates the records, groups TUs by CTB, cuts PUs into MC tiles and packs everything into `hb`
-// (which must hold L->total bytes; call with hb == nullptr first to size it).
-// Section order in the staging buffer / device arena: the raw record arrays first (their offsets depend only on the
-// counts, so copying them can start before the work lists exist), then the lists the planner builds.
-//   0 pus, 1 weights, 2 tus, 5 coeffs, 6 slices, 7 ctbs, 8 bs_map, 9 qp_map, 10 nofilt_map, 11 scaling |
-//   3 list_a (non-intra TU indices by k_residual class), 4 list_b (intra TU indices by task), 12 MC units / tiles, 13 task_start
-static const int k_raw_sections[10] = {0, 1, 2, 5, 6, 7, 8, 9, 10, 11};
-static const int k_list_sections[4] = {3, 4, 12, 13};
-
-static int plan_begin(b200_engine* en, const b200_picture* pic, PicLayout* L, size_t* cap_total)
-{
-  const b200_pic_params& p = pic->params;
-  int rc = check_params(p);
-  if (rc) return rc;
-  if ((pic->n_pu && !pic->pus) || (pic->n_tu && !pic->tus) || (pic->n_coeff && !pic->coeffs) || !pic->slices || !pic->ctbs || !pic->qp_map ||
-      !pic->nofilt_map || pic->n_slices == 0)
-    return set_err(B200_ERR_INVALID, "missing record arrays");
-  if (pic->n_pu >= (1u << 20)) return set_err(B200_ERR_INVALID, "too many PUs");
-  const int S = 1 << p.log2_ctb_size;
-  const int wctb = (p.width + S - 1) / S, hctb = (p.height + S - 1) / S, n_ctb = wctb * hctb;
-  const int w4 = (p.width + 3) / 4, h4 = (p.height + 3) / 4, w8 = (p.width + 7) / 8, h8 = (p.height + 7) / 8;
-  L->params = p;
-  L->n_tu = pic->n_tu;
-  L->has_scaling = pic->scaling_factors != nullptr;
-  L->run_deblock = !(p.flags & B200_PIC_SKIP_DEBLOCK) && pic->bs_map && (p.stop_after_stage == B200_STAGE_ALL || p.stop_after_stage == B200_STAGE_DEBLOCK);
-  L->run_sao = (p.flags & B200_PIC_SAO_ENABLED) && !(p.flags & B200_PIC_SKIP_SAO) && p.stop_after_stage == B200_STAGE_ALL;
-
-  for (int i = 0; i < n_ctb; i++)
-    if (pic->ctbs[i].slice_idx >= pic->n_slices) return set_err(B200_ERR_INVALID, "CTB %d slice index", i);
-  size_t sz[14] = {};
-  sz[0] = sizeof(b200_pu) * pic->n_pu;
-  sz[1] = sizeof(b200_weight_entry) * pic->n_weights;
-  sz[2] = sizeof(b200_tu) * pic->n_tu;
-  sz[5] = sizeof(b200_coeff) * pic->n_coeff;
-  sz[6] = sizeof(b200_slice_info) * pic->n_slices;
-  sz[7] = sizeof(b200_ctb_info) * (size_t)n_ctb;
-  sz[8] = L->run_deblock ? (size_t)w4 * h4 : 0;
-  sz[9] = (size_t)w8 * h8;
-  sz[10] = (size_t)w8 * h8;
-  sz[11] = L->has_scaling ? B200_SCALING_FACTOR_BYTES : 0;
-  size_t total = 0;
-  for (int i : k_raw_sections) { L->off[i] = total; total += align_up(sz[i], 256); }
-  L->raw_total = total;
-  L->direct = (p.flags & B200_PIC_RECORDS_PINNED) != 0;
-  const void* src[14] = {pic->pus, pic->weights, pic->tus, nullptr, nullptr, pic->coeffs, pic->slices, pic->ctbs, pic->bs_map, pic->qp_map, pic->nofilt_map,
-                         pic->scaling_factors, nullptr, nullptr};
-  for (int i : k_raw_sections) { L->raw_src[i] = src[i]; L->raw_sz[i] = sz[i]; }
-  // upper bound of the lists: every TU in one list, one task per TU; MC units cannot outnumber 4x8 blocks unless PUs overlap
-  L->unit_cap = ((size_t)w4 * h4 / 2 + 64 + 8 * MCT_MAX_TILES) * 3 / 2 + 64;  // + the padding of the class-pure batches + the batch table
-  *cap_total = total + 3 * align_up(sizeof(uint32_t) * ((size_t)pic->n_tu + 1), 256) + align_up(sizeof(uint32_t) * L->unit_cap, 256) + 256;
-  return B200_OK;
-}
-
-// PU validation + MC work list for the PU range [i0, i1) into the part's own tile list (parts run on pool threads;
-// plan_pus_merge sorts them into class-pure batches)
-static int plan_pus_part(b200_engine* en, const b200_picture* pic, int part, uint32_t i0, uint32_t i1)
-{
-  const b200_pic_params& p = pic->params;
-  std::vector<uint32_t>& tiles = en->pu_tiles[part];
-  // at most 16 tiles (64x64 PU) per record: written through a raw pointer, trimmed at the end (no per-tile capacity check)
-  tiles.resize((size_t)(i1 - i0) * 16);
-  uint32_t* out = tiles.data();
-  uint32_t ref_mask = 0;
-  size_t count[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  const bool wide = p.bit_depth_luma > 8;  // same rule as the launch_picture<P> dispatch
-  const bool legacy = en->mc_legacy;
-  const unsigned pw = p.width, ph = p.height;
-  const uint32_t n_weights = pic->n_weights;
-  const b200_pu* pus = pic->pus;
-  for (uint32_t i = i0; i < i1; i++) {
-    const b200_pu& pu = pus[i];
-    const unsigned w = pu.w, h = pu.h;
-    if (w - 1u > 63u || h - 1u > 63u || ((w | h | pu.x | pu.y) & 3u) || pu.x + w > pw || pu.y + h > ph)
-      return set_err(B200_ERR_INVALID, "PU %u out of range", i);
-    if ((pu.flags & B200_PU_WEIGHTED) && pu.wt_idx >= n_weights) return set_err(B200_ERR_INVALID, "PU %u weight index", i);
-    if (pu.ref_slot[0] >= B200_MAX_SLOTS || pu.ref_slot[1] >= B200_MAX_SLOTS) return set_err(B200_ERR_INVALID, "PU %u reference slot", i);
-    const unsigned l0 = pu.flags & B200_PU_PRED_L0, l1 = pu.flags & B200_PU_PRED_L1;
-    if (!(l0 | l1)) continue;
-    if (l0 && pu.ref_slot[0] >= 0) ref_mask |= 1u << pu.ref_slot[0];
-    if (l1 && pu.ref_slot[1] >= 0) ref_mask |= 1u << pu.ref_slot[1];
-    if (wide) {  // 16-bit path: <= 16x16 tiles, one warp each (kernels_mc.cuh)
-      for (unsigned ty = 0; ty * MC_TILE < h; ty++)
-        for (unsigned tx = 0; tx * MC_TILE < w; tx++) *out++ = i | (tx << 20) | (ty << 22);
-    } else if (legacy) {  // first-generation 8-bit path: <= 8x16 units, one quarter-warp each (kernels_mc8.cuh)
-      tiles.resize((size_t)(out - tiles.data()));  // (rare debug path: up to 32 units per PU, keep the simple form)
-      for (unsigned uy = 0; uy * MC8_UH < h; uy++)
-        for (unsigned ux = 0; ux * MC8_UW < w; ux++) tiles.push_back(MC8_UNIT(i, ux, uy));
-      const size_t used = tiles.size();
-      tiles.resize(used + (size_t)(i1 - i - 1) * 32 + 32);
-      out = tiles.data() + used;
-    } else {     // 8-bit path: <= 16x16 tiles with their class (kernels_mct.cuh), sorted into class-pure batches by the merge
-      const unsigned bi = (l0 && l1) ? MCT_CLASS_BI : 0;
-      for (unsigned ty = 0; ty * 16 < h; ty++) {
-        const unsigned tall = (h - 16 * ty > 8) ? MCT_CLASS_TALL : 0;
-        for (unsigned tx = 0; tx * 16 < w; tx++) {
-          const unsigned cls = bi | tall | ((w - 16 * tx > 8) ? MCT_CLASS_WIDE : 0);
-          *out++ = MCT_TILE_WORD(i, tx, ty, cls);
-          count[cls]++;
-        }
-      }
-    }
-  }
-  tiles.resize((size_t)(out - tiles.data()));
-  for (int c = 0; c < 8; c++) en->pu_count[part][c] = count[c];
-  en->pu_ref_mask[part] = ref_mask;
-  return B200_OK;
-}
-
-// Concatenates the parts; 8-bit: counting sort by class, every class padded to whole batches (MCT_CLASS_TILES tiles of one class,
-// padding = MCT_INVALID), the batch table (first tile index | class) behind the tile words in the same section.
-static int plan_pus_merge(b200_engine* en, const b200_picture* pic, PicLayout* L)
-{
-  const bool wide = pic->params.bit_depth_luma > 8;
-  std::vector<uint32_t>& tiles = en->tiles;
-  L->n_batches = 0;
-  for (int part = 0; part < PLAN_PU_PARTS; part++) L->ref_mask |= en->pu_ref_mask[part];
-  size_t n_words;
-  if (wide || en->mc_legacy) {
-    tiles.clear();
-    for (int part = 0; part < PLAN_PU_PARTS; part++) tiles.insert(tiles.end(), en->pu_tiles[part].begin(), en->pu_tiles[part].end());
-    n_words = tiles.size();
-  } else {
-    size_t count[8] = {}, start[8], total = 0, nb = 0;
-    for (int part = 0; part < PLAN_PU_PARTS; part++)
-      for (int c = 0; c < 8; c++) count[c] += en->pu_count[part][c];
-    for (int c = 0; c < 8; c++) {
-      const size_t per = MCT_CLASS_TILES(c), batches = (count[c] + per - 1) / per;
-      start[c] = total;
-      total += batches * per;
-      nb += batches;
-    }
-    tiles.assign(total + nb, MCT_INVALID);
-    size_t bi = total;
-    for (int c = 0; c < 8; c++)
-      for (size_t f = start[c]; f < start[c] + (count[c] + MCT_CLASS_TILES(c) - 1) / MCT_CLASS_TILES(c) * MCT_CLASS_TILES(c); f += MCT_CLASS_TILES(c))
-        tiles[bi++] = MCT_BATCH_WORD(f, c);
-    for (int part = 0; part < PLAN_PU_PARTS; part++)
-      for (uint32_t t : en->pu_tiles[part]) tiles[start[(t >> 24) & 7]++] = t;
-    n_words = total;
-    L->n_batches = (int)nb;
-  }
-  if (tiles.size() > L->unit_cap) return set_err(B200_ERR_INVALID, "PUs overlap (more MC units than the picture has 4x8 blocks)");
-  L->n_tiles = (int)n_words;  // tile words; en->tiles also holds the n_batches batch words behind them
-  return B200_OK;
-}
-
-// TU validation + the k_residual work classes for the TU range [i0, i1) into the part's own lists (two parts run on pool
-// threads; plan_and_pack concatenates them).  Classes: warp per TU (16x16, 32x32, PCM) | quarter-warp per 8x8 | lane per 4x4.
-#define PLAN_TU_PARTS PLAN_INTRA_PARTS  // validation and the intra task formation share one pass over a range of TUs
-// One TU record against the picture; B200_OK or the error (message set).  `dims`: plane sizes per cIdx (0 when the plane does not exist).
-struct TuDims { int pw[3], ph[3]; };
-static inline TuDims tu_dims(const b200_pic_params& p)
-{
-  TuDims d;
-  d.pw[0] = p.width; d.ph[0] = p.height;
-  d.pw[1] = d.pw[2] = p.chroma_format_idc ? p.width / 2 : 0;
-  d.ph[1] = d.ph[2] = p.chroma_format_idc ? p.height / 2 : 0;
-  return d;
-}
-static inline int tu_check(const TuDims& d, const b200_picture* pic, uint32_t i, const b200_tu& tu)
-{
-  const unsigned l2 = tu.log2_size, c = tu.cidx;
-  if (l2 - 2u > 3u || c > 2u) return set_err(B200_ERR_INVALID, "TU %u out of range", i);
-  const int nT = 1 << l2, pw = d.pw[c], ph = d.ph[c];
-  if (tu.x + nT > pw || tu.y + nT > ph || ((tu.x | tu.y) & (nT - 1))) return set_err(B200_ERR_INVALID, "TU %u out of range", i);  // nT >= 4: also the 4-sample grid
-  if ((size_t)tu.coeff_off + tu.n_coeff > pic->n_coeff || tu.n_coeff > nT * nT) return set_err(B200_ERR_INVALID, "TU %u coefficient range", i);
-  if ((tu.flags & B200_TU_PCM) && tu.n_coeff != nT * nT) return set_err(B200_ERR_INVALID, "PCM TU %u sample count", i);
-  if (tu.flags & B200_TU_INTRA) {
-    if (tu.intra_mode > 34) return set_err(B200_ERR_INVALID, "TU %u intra mode", i);
-    // avail bits must name samples inside the picture (k_intra reads the border and the pending flags at those positions)
-    const int half = nT >> 1;  // groups of 4 samples per side
-    const uint32_t gm = half >= 32 ? 0xffffffffu : (1u << half) - 1u;
-    const uint32_t left = (uint32_t)tu.avail & 0xffffu, top = (uint32_t)(tu.avail >> B200_AVAIL_TOP_BIT0) & 0xffffu;
-    const bool corner = (tu.avail >> B200_AVAIL_CORNER_BIT) & 1;
-    const int rows_below = (ph - tu.y) >> 2, cols_right = (pw - tu.x) >> 2;  // groups that still lie inside the plane
-    const uint32_t lm = rows_below >= 16 ? 0xffffu : (1u << rows_below) - 1u, tm = cols_right >= 16 ? 0xffffu : (1u << cols_right) - 1u;
-    if ((left & ~gm) || (top & ~gm) || (tu.avail >> (B200_AVAIL_TOP_BIT0 + 16)) || (left && tu.x == 0) || (top && tu.y == 0) ||
-        (corner && (tu.x == 0 || tu.y == 0)) || (left & ~lm) || (top & ~tm))
-      return set_err(B200_ERR_INVALID, "TU %u intra availability names samples outside the picture", i);
-  }
-  return B200_OK;
-}
-
-// TU validation, the k_residual classes of the non-intra TUs and the intra work list, in one pass over the TU records.  Intra tasks: the TUs of one plane inside one aligned 16x16-luma / 8x8-chroma region (contiguous per plane in
-// decode order); a TU at least as large as the region is a task of its own.  Tasks are emitted in a topological order: CTB
-// anti-diagonal x + 2y, ties in decode order.  The TU list is cut at CTB boundaries into PLAN_INTRA_PARTS ranges (a region
-// never crosses a CTB, so no task spans two ranges) and the phases A, C, E run per range on the pool threads:
-//   A  per range: intra TUs, their (range-local) task ids, tasks per diagonal          B  serial: task / rank offsets of the ranges
-//   C  per range: rank of every task, TUs per task                                      D  serial: prefix sum -> task_start
-//   E  per range: list_b (TU indices grouped by task in rank order)
-
-static inline size_t plan_diag_of(const b200_pic_params& p, const b200_tu& tu)
-{
-  const int sh = tu.cidx ? 1 : 0;
-  return (size_t)((tu.x << sh) >> p.log2_ctb_size) + 2 * (size_t)((tu.y << sh) >> p.log2_ctb_size);
-}
-static inline uint32_t plan_ctb_of(const b200_pic_params& p, const b200_tu& tu)
-{
-  const int sh = (tu.cidx && tu.cidx <= 2) ? 1 : 0;
-  return (uint32_t)(((uint32_t)tu.x << sh) >> p.log2_ctb_size) | ((uint32_t)(((uint32_t)tu.y << sh) >> p.log2_ctb_size) << 16);
-}
-
-static void plan_intra_ranges(b200_engine* en, const b200_picture* pic)
-{
-  const b200_pic_params& p = pic->params;
-  uint32_t prev = 0;
-  for (int k = 0; k < PLAN_INTRA_PARTS; k++) {
-    uint32_t end = (k == PLAN_INTRA_PARTS - 1) ? pic->n_tu : (uint32_t)((uint64_t)pic->n_tu * (k + 1) / PLAN_INTRA_PARTS);
-    if (end < prev) end = prev;
-    // move the cut forward to the next CTB change (all TUs of a CTB are contiguous in decode order)
-    while (end > 0 && end < pic->n_tu && plan_ctb_of(p, pic->tus[end]) == plan_ctb_of(p, pic->tus[end - 1])) end++;
-    en->ipart[k].i0 = prev;
-    en->ipart[k].i1 = end;
-    prev = end;
-  }
-}
-
-static int plan_intra_A(b200_engine* en, const b200_picture* pic, int k, int n_diag, int wctb, int hctb)
-{
-  const b200_pic_params& p = pic->params;
-  IntraPart& ip = en->ipart[k];
-  std::vector<uint32_t>&la = en->part_a[k][0], &la8 = en->part_a[k][1], &la4 = en->part_a[k][2];  // non-intra TUs with a residual, by k_residual class
-  la.clear();
-  la8.clear();
-  la4.clear();
-  ip.intra_idx.clear();
-  ip.task_of.clear();
-  ip.task_first.clear();
-  ip.task_cell.clear();
-  ip.diag_cnt.assign((size_t)n_diag, 0);
-  // Pictures with inter prediction have few, scattered intra blocks: the per-task overhead of k_intra dominates there, so the
-  // small TUs of ALL planes of a region form one task (luma, then Cb, then Cr) when they are at most 16; intra pictures keep
-  // one task per plane (three shorter dependency chains side by side).
-  const bool merged = pic->n_pu > 0 && !en->intra_split_planes;
-  const int lg_region = en->region == 16 ? 4 : 3;
-  const TuDims dims = tu_dims(p);
-  long long cur_key[3] = {-1, -1, -1};
-  uint32_t cur_task[3] = {0, 0, 0};
-  uint32_t run[48];  // merged mode: the small intra TUs of the current region (at most 16 + 4 + 4, sized generously)
-  int n_run = 0;
-  long long run_key = -1;
-  auto new_task = [&](uint32_t first_tu) {
-    const b200_tu& ft = pic->tus[first_tu];
-    ip.task_first.push_back(first_tu);
-    ip.diag_cnt[plan_diag_of(p, ft)]++;
-    const uint32_t sh = ft.cidx ? 1 : 0;  // what plan_intra_levels needs of the task, kept here so that pass reads no TU record
-    const uint32_t R = std::max(1u, ((1u << ft.log2_size) << sh) >> lg_region);
-    ip.task_cell.push_back((((uint32_t)ft.x << sh) >> lg_region) | ((((uint32_t)ft.y << sh) >> lg_region) << 12) | (R << 24) | ((uint32_t)ft.cidx << 28));
-    return (uint32_t)ip.task_first.size() - 1;
-  };
-  auto flush_run = [&]() {
-    if (!n_run) return;
-    int cnt[3] = {0, 0, 0};
-    for (int j = 0; j < n_run; j++) cnt[pic->tus[run[j]].cidx]++;
-    const bool one = n_run <= 16;
-    uint32_t t = 0;
-    if (one) t = new_task(run[0]);
-    for (int c = 0; c < 3; c++) {  // plane by plane, decode order inside a plane
-      if (!cnt[c]) continue;
-      bool first = true;
-      for (int j = 0; j < n_run; j++) {
-        if (pic->tus[run[j]].cidx != c) continue;
-        if (!one && first) t = new_task(run[j]);
-        first = false;
-        ip.intra_idx.push_back(run[j]);
-        ip.task_of.push_back(t);
-      }
-    }
-    n_run = 0;
-  };
-  for (uint32_t i = ip.i0; i < ip.i1; i++) {
-    const b200_tu& tu = pic->tus[i];
-    if (const int rc = tu_check(dims, pic, i, tu)) return rc;
-    if (!(tu.flags & B200_TU_INTRA)) {
-      if (tu.flags & (B200_TU_CBF | B200_TU_PCM)) {
-        if ((tu.flags & B200_TU_PCM) || tu.log2_size > 3) la.push_back(i);
-        else if (tu.log2_size == 3) la8.push_back(i);
-        else la4.push_back(i);
-      }
-      continue;
-    }
-    const int c = tu.cidx, G = en->region >> (c ? 1 : 0), nT = 1 << tu.log2_size;
-    if (merged) {
-      if (nT >= G) {  // a TU at least as large as the region is a task of its own
-        flush_run();
-        run_key = -1;
-        ip.intra_idx.push_back(i);
-        ip.task_of.push_back(new_task(i));
-        continue;
-      }
-      const int sh = c ? 1 : 0;
-      const long long key = (((long long)((tu.y << sh) >> lg_region)) << 20) | ((tu.x << sh) >> lg_region);
-      if (key != run_key || n_run == 48) {
-        flush_run();
-        run_key = key;
-      }
-      run[n_run++] = i;
-      continue;
-    }
-    ip.intra_idx.push_back(i);
-    const long long key = (nT >= G) ? -2 - (long long)i : (((long long)(tu.y >> (lg_region - (c ? 1 : 0)))) << 20) | (tu.x >> (lg_region - (c ? 1 : 0)));
-    if (key != cur_key[c]) {
-      cur_key[c] = key;
-      cur_task[c] = new_task(i);
-    }
-    ip.task_of.push_back(cur_task[c]);
-  }
-  flush_run();
-  return B200_OK;
-}
-
-static void plan_intra_B(b200_engine* en, int n_diag, uint32_t* n_task, uint32_t* n_intra)
-{
-  uint32_t nt = 0, ni = 0;
-  for (int k = 0; k < PLAN_INTRA_PARTS; k++) {
-    en->ipart[k].task_base = nt;
-    nt += (uint32_t)en->ipart[k].task_first.size();
-    ni += (uint32_t)en->ipart[k].intra_idx.size();
-    en->ipart[k].diag_off.assign((size_t)n_diag, 0);
-  }
-  uint32_t run = 0;
-  for (int d = 0; d < n_diag; d++)
-    for (int k = 0; k < PLAN_INTRA_PARTS; k++) {  // ranges are in decode order: within a diagonal, earlier ranges rank first
-      en->ipart[k].diag_off[d] = run;
-      run += en->ipart[k].diag_cnt[d];
-    }
-  *n_task = nt;
-  *n_intra = ni;
-  en->task_order.resize(nt);
-  en->task_start.assign((size_t)nt + 1, 0);
-  en->list_b.resize(ni);
-}
-
-// Ticket order by DAG LEVEL (default; B200_INTRA_ORDER=diag keeps the CTB anti-diagonal order).  A level is assigned per task in
-// ONE pass over the tasks in decode order through a map "region cell (16x16 luma) -> highest level of a task covering it":
-//   level(task) = 1 + max over the cells its TUs may read (the column left of it from one cell above to 2x its height below —
-//   corner, left and bottom-left neighbours — and the row above it to 2x its width — top and top-right), cells not written yet
-//   (decoded later, or not intra) count 0.
-// That is a superset of the true dependencies (availability bits), which is all a valid layering needs: every neighbour a task
-// waits for has a lower level.  Tasks of one level are independent, so with tickets sorted by level the lowest unfinished
-// tickets are exactly the ready tasks: the persistent warps of k_intra hold ready work instead of spinning on tasks far down
-// the anti-diagonal, and the grid is sized to the DAG's width (the widest level) instead of the whole GPU — the other SMs stay
-// free for the pictures it overlaps with.  (The anti-diagonal order is topological too, but of the ~500 consecutive tickets
-// the warps hold only the first task of every CTB chain is ready.)  Intra pictures keep one map per plane (their tasks are
-// per plane); pictures with inter prediction one map (tasks span the planes).
-static void plan_intra_levels(b200_engine* en, const b200_picture* pic, PicLayout* L, uint32_t n_task)
-{
-  const b200_pic_params& p = pic->params;
-  const int lg = en->region == 16 ? 4 : 3;
-  const int cw = (p.width + (1 << lg) - 1) >> lg, ch = (p.height + (1 << lg) - 1) >> lg;
-  const bool per_plane = pic->n_pu == 0 || en->intra_split_planes;
-  for (int c = 0; c < (per_plane ? 3 : 1); c++) en->cell_level[c].assign((size_t)cw * ch, 0);
-  std::vector<uint32_t>& level = en->task_level;
-  level.resize(n_task);
-  uint32_t max_level = 0;
-  for (int k = 0; k < PLAN_INTRA_PARTS; k++) {
-    const IntraPart& ip = en->ipart[k];
-    for (size_t t = 0; t < ip.task_first.size(); t++) {
-      const uint32_t tc = ip.task_cell[t];
-      const int cx = (int)(tc & 0xfff), cy = (int)((tc >> 12) & 0xfff);
-      const int R = (int)((tc >> 24) & 0xf);  // cells per side: 1 (region task) or the large TU's size
-      uint32_t* map = en->cell_level[per_plane ? (tc >> 28) : 0].data();
-      uint32_t lvl = 0;
-      if (cx > 0)
-        for (int y = std::max(cy - 1, 0); y < std::min(cy + 2 * R, ch); y++) lvl = std::max(lvl, map[(size_t)y * cw + cx - 1]);
-      if (cy > 0)
-        for (int x = cx; x < std::min(cx + 2 * R, cw); x++) lvl = std::max(lvl, map[(size_t)(cy - 1) * cw + x]);
-      lvl++;
-      level[ip.task_base + t] = lvl;
-      if (lvl > max_level) max_level = lvl;
-      for (int y = cy; y < std::min(cy + R, ch); y++)
-        for (int x = cx; x < std::min(cx + R, cw); x++) {
-          uint32_t& m = map[(size_t)y * cw + x];
-          if (lvl > m) m = lvl;  // several tasks may cover a cell (planes of a merged region that were split, large chroma TUs)
-        }
-    }
-  }
-  // rank = position in (level, decode order): counting sort over the levels; the widest level sizes the grid
-  std::vector<uint32_t>& off = en->level_off;
-  off.assign((size_t)max_level + 2, 0);
-  for (uint32_t t = 0; t < n_task; t++) off[level[t] + 1]++;
-  uint32_t width = 0;
-  for (size_t l = 1; l < off.size(); l++) {
-    if (off[l] > width) width = off[l];
-    off[l] += off[l - 1];
-  }
-  uint32_t* order = en->task_order.data();
-  for (uint32_t t = 0; t < n_task; t++) order[t] = off[level[t]]++;
-  L->intra_levels = (int)max_level;
-  L->intra_width = (int)width;
-}
-
-static void plan_intra_C(b200_engine* en, const b200_picture* pic, int k, bool by_level)
-{
-  const b200_pic_params& p = pic->params;
-  IntraPart& ip = en->ipart[k];
-  uint32_t* order = en->task_order.data() + ip.task_base;
-  if (!by_level)
-    for (size_t t = 0; t < ip.task_first.size(); t++) order[t] = ip.diag_off[plan_diag_of(p, pic->tus[ip.task_first[t]])]++;
-  uint32_t* ts = en->task_start.data();
-  for (size_t j = 0; j < ip.task_of.size(); j++) ts[order[ip.task_of[j]] + 1]++;  // a task belongs to exactly one range: no two threads touch one entry
-}
-
-static void plan_intra_E(b200_engine* en, int k)
-{
-  IntraPart& ip = en->ipart[k];
-  const uint32_t* order = en->task_order.data() + ip.task_base;
-  const uint32_t* ts = en->task_start.data();
-  ip.fill.resize(ip.task_first.size());
-  for (size_t t = 0; t < ip.task_first.size(); t++) ip.fill[t] = ts[order[t]];
-  uint32_t* lb = en->list_b.data();
-  for (size_t j = 0; j < ip.intra_idx.size(); j++) lb[ip.fill[ip.task_of[j]]++] = ip.intra_idx[j];
-}
-
-// Runs `f(k)` for k = 0..n-1 on the pool (or inline without one) and waits.
-template <typename F>
-static void plan_parallel(b200_engine* en, int n, F f)
-{
-  for (int k = 0; k < n; k++) en->prun([=] { f(k); });
-  en->pwait();
-}
-
-// The serial glue of the intra planner after phase A has run for every range (also used by plan_and_pack, where phase A runs
-// next to the other planning work).
-static void plan_intra_finish(b200_engine* en, const b200_picture* pic, PicLayout* L, int n_diag)
-{
-  uint32_t n_task = 0, n_intra = 0;
-  plan_intra_B(en, n_diag, &n_task, &n_intra);
-  const bool by_level = n_task && (en->intra_level_order == 2 || (en->intra_level_order == 1 && pic->n_pu == 0));
-  L->intra_levels = L->intra_width = 0;
-  if (by_level) plan_intra_levels(en, pic, L, n_task);
-  plan_parallel(en, PLAN_INTRA_PARTS, [=](int k) { plan_intra_C(en, pic, k, by_level); });
-  uint32_t* ts = en->task_start.data();
-  for (uint32_t t = 0; t < n_task; t++) ts[t + 1] += ts[t];
-  plan_parallel(en, PLAN_INTRA_PARTS, [=](int k) { plan_intra_E(en, k); });
-  L->n_task = (int)n_task;
-  L->n_b = (int)n_intra;
-}
-
-static void plan_finish(PicLayout* L)
-{
-  size_t sz[14] = {};
-  sz[3] = sizeof(uint32_t) * (size_t)L->n_a;
-  sz[4] = sizeof(uint32_t) * (size_t)L->n_b;
-  sz[12] = sizeof(uint32_t) * (size_t)(L->n_tiles + L->n_batches);
-  sz[13] = L->n_task ? sizeof(uint32_t) * (size_t)(L->n_task + 1) : 0;
-  size_t total = L->raw_total;
-  for (int i : k_list_sections) { L->off[i] = total; total += align_up(sz[i], 256); }
-  L->total = total ? total : 256;
-}
-
-// part 0..2: the raw record arrays in three roughly equal shares (pool threads)
-static void pack_raw(const b200_picture* pic, const PicLayout& L, uint8_t* hb, int part)
-{
-  const b200_pic_params& p = pic->params;
-  const size_t* off = L.off;
-  const int S = 1 << p.log2_ctb_size;
-  const int wctb = (p.width + S - 1) / S, hctb = (p.height + S - 1) / S, n_ctb = wctb * hctb;
-  const int w4 = (p.width + 3) / 4, h4 = (p.height + 3) / 4, w8 = (p.width + 7) / 8, h8 = (p.height + 7) / 8;
-  if (part == 0) {
-    if (pic->n_coeff) memcpy(hb + off[5], pic->coeffs, sizeof(b200_coeff) * pic->n_coeff);
-  } else if (part == 1) {
-    if (pic->n_tu) memcpy(hb + off[2], pic->tus, sizeof(b200_tu) * pic->n_tu);
-    memcpy(hb + off[6], pic->slices, sizeof(b200_slice_info) * pic->n_slices);
-    memcpy(hb + off[7], pic->ctbs, sizeof(b200_ctb_info) * (size_t)n_ctb);
-  } else {
-    if (pic->n_pu) memcpy(hb + off[0], pic->pus, sizeof(b200_pu) * pic->n_pu);
-    if (pic->n_weights) memcpy(hb + off[1], pic->weights, sizeof(b200_weight_entry) * pic->n_weights);
-    if (L.run_deblock) memcpy(hb + off[8], pic->bs_map, (size_t)w4 * h4);
-    memcpy(hb + off[9], pic->qp_map, (size_t)w8 * h8);
-    memcpy(hb + off[10], pic->nofilt_map, (size_t)w8 * h8);
-    if (L.has_scaling) memcpy(hb + off[11], pic->scaling_factors, B200_SCALING_FACTOR_BYTES);
-  }
-}
-
-static void pack_lists(b200_engine* en, const PicLayout& L, uint8_t* hb)
-{
-  const size_t* off = L.off;
-  if (L.n_a) memcpy(hb + off[3], en->list_a.data(), sizeof(uint32_t) * (size_t)L.n_a);
-  if (L.n_b) memcpy(hb + off[4], en->list_b.data(), sizeof(uint32_t) * (size_t)L.n_b);
-  if (L.n_task) memcpy(hb + off[13], en->task_start.data(), sizeof(uint32_t) * (size_t)(L.n_task + 1));
-  if (L.n_tiles) memcpy(hb + off[12], en->tiles.data(), sizeof(uint32_t) * (size_t)(L.n_tiles + L.n_batches));
-}
-
 // cap_hint = the largest staging capacity any set of the engine has needed: a set that has to grow goes straight to it, so that
 // every set is reallocated at most once after the first large (intra) picture instead of whenever such a picture happens to land
 // on it (page-locking tens of MB and cudaFree both stall the other threads' CUDA calls).
@@ -1419,63 +872,19 @@ static int ensure_staging(StagingSet& ss, size_t total)
   return B200_OK;
 }
 
-// list_a = class by class (warp | 8x8 | 4x4), the validation parts in order
-static void merge_list_a(b200_engine* en, PicLayout* L)
-{
-  std::vector<uint32_t>& la = en->list_a;
-  la.clear();
-  for (int cls = 0; cls < 3; cls++) {
-    for (int part = 0; part < PLAN_TU_PARTS; part++) la.insert(la.end(), en->part_a[part][cls].begin(), en->part_a[part][cls].end());
-    if (cls == 0) L->n_aw = (int)la.size();
-    if (cls == 1) L->n_a8 = (int)la.size() - L->n_aw;
-  }
-  L->n_a = (int)la.size();
-}
-
-// Host side of one picture: validate, build the work lists, fill the pinned staging buffer.  The raw record arrays are
-// copied by pool threads and the PUs are planned on a pool thread while this thread plans the TUs.
-static int plan_and_pack(b200_engine* en, const b200_picture* pic, PicLayout* L, StagingSet& ss, double* t_plan_pack)
+// Host side of one picture: validate, build the work lists, fill the pinned staging buffer (plan_build: on the planner's pool).
+static int plan_and_pack(Planner& pl, const b200_picture* pic, PicLayout* L, StagingSet& ss, double* t_plan_pack)
 {
   auto now = [] { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
   const double t0 = now();
   size_t cap = 0;
-  int rc = plan_begin(en, pic, L, &cap);
+  int rc = plan_begin(pl, pic, L, &cap);
   if (rc) return rc;
   rc = ensure_staging(ss, cap);
   if (rc) return rc;
   const double t1 = now();
-  uint8_t* hb = ss.host;
-  const b200_pic_params& pp = pic->params;
-  const int S = 1 << pp.log2_ctb_size, wctb = (pp.width + S - 1) / S, hctb = (pp.height + S - 1) / S, n_diag = wctb + 2 * hctb;
-  en->use_helper = en->helper && pic->n_tu > 200000;  // shadow engines: see b200_engine::helper
-  int rc_pu[PLAN_PU_PARTS] = {}, rc_tv[PLAN_TU_PARTS] = {};
-  std::string err_pu[PLAN_PU_PARTS], err_tv[PLAN_TU_PARTS];
-  plan_intra_ranges(en, pic);
-  for (int k = 0; k < PLAN_INTRA_PARTS; k++)  // the longest items first: TU validation + residual classes + intra tasks of one range
-    en->prun([&, k] {
-      rc_tv[k] = plan_intra_A(en, pic, k, n_diag, wctb, hctb);
-      if (rc_tv[k]) err_tv[k] = g_err;  // the worker's thread-local message
-    });
-  for (int part = 0; part < PLAN_PU_PARTS; part++) {
-    const uint32_t i0 = (uint32_t)((uint64_t)pic->n_pu * part / PLAN_PU_PARTS), i1 = (uint32_t)((uint64_t)pic->n_pu * (part + 1) / PLAN_PU_PARTS);
-    en->prun([&, part, i0, i1] {
-      rc_pu[part] = plan_pus_part(en, pic, part, i0, i1);
-      if (rc_pu[part]) err_pu[part] = g_err;  // the worker's thread-local message
-    });
-  }
-  if (!L->direct)
-    for (int part = 0; part < 3; part++) en->prun([=] { pack_raw(pic, *L, hb, part); });
-  en->pwait();
-  for (int part = 0; part < PLAN_TU_PARTS; part++)
-    if (rc_tv[part]) return set_err(rc_tv[part], "%s", err_tv[part].c_str());
-  for (int part = 0; part < PLAN_PU_PARTS; part++)
-    if (rc_pu[part]) return set_err(rc_pu[part], "%s", err_pu[part].c_str());
-  plan_intra_finish(en, pic, L, n_diag);
-  merge_list_a(en, L);
-  rc = plan_pus_merge(en, pic, L);
+  rc = plan_build(pl, pic, L, ss.host);
   if (rc) return rc;
-  plan_finish(L);
-  pack_lists(en, *L, hb);
   if (t_plan_pack) { t_plan_pack[0] = t1 - t0; t_plan_pack[1] = now() - t1; }
   return B200_OK;
 }
@@ -1484,63 +893,23 @@ extern "C" int b200_plan_picture_host(const b200_picture* pic, uint32_t counts[8
                                       uint32_t* list_b, size_t cap_b, uint32_t* task_start, size_t cap_tasks)
 {
   if (!pic || !counts) return set_err(B200_ERR_INVALID, "null argument");
-  b200_engine* en = new (std::nothrow) b200_engine();  // no CUDA call is made on this path
-  if (!en) return set_err(B200_ERR_NOMEM, "out of memory");
-  if (const char* e = getenv("B200_REGION")) en->region = (atoi(e) == 8) ? 8 : 16;
-  if (const char* e = getenv("B200_INTRA_ORDER")) en->intra_level_order = !strcmp(e, "diag") ? 0 : !strcmp(e, "level_i") ? 1 : 2;
+  Planner pl;  // no pool, no CUDA call
+  pl.opt = plan_options_from_env();
   PicLayout L;
   size_t cap = 0;
-  auto now = [] { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
-  const bool prof = getenv("B200_HOST_PROF") != nullptr;
-  double t[5] = {now(), 0, 0, 0, 0};
-  int rc = plan_begin(en, pic, &L, &cap);
-  t[1] = now();
-  for (int part = 0; part < PLAN_PU_PARTS && !rc; part++)
-    rc = plan_pus_part(en, pic, part, (uint32_t)((uint64_t)pic->n_pu * part / PLAN_PU_PARTS), (uint32_t)((uint64_t)pic->n_pu * (part + 1) / PLAN_PU_PARTS));
-  if (!rc) rc = plan_pus_merge(en, pic, &L);
-  t[2] = now();
-  t[3] = now();
-  if (!rc) {
-    const b200_pic_params& pp = pic->params;
-    const int S = 1 << pp.log2_ctb_size, wctb = (pp.width + S - 1) / S, hctb = (pp.height + S - 1) / S, n_diag = wctb + 2 * hctb;
-    plan_intra_ranges(en, pic);
-    for (int k = 0; k < PLAN_INTRA_PARTS && !rc; k++) rc = plan_intra_A(en, pic, k, n_diag, wctb, hctb);
-    if (!rc) plan_intra_finish(en, pic, &L, n_diag);
-  }
-  t[4] = now();
-  if (prof) {
-    double u[4];
-    u[0] = now();
-    for (int part = 0; part < PLAN_PU_PARTS && !rc; part++) en->pu_ref_mask[part] = 0;
-    if (!rc) rc = plan_pus_merge(en, pic, &L);
-    u[1] = now();
-    if (!rc) {
-      const b200_pic_params& pp = pic->params;
-      const int S = 1 << pp.log2_ctb_size, wctb = (pp.width + S - 1) / S, hctb = (pp.height + S - 1) / S;
-      plan_intra_finish(en, pic, &L, wctb + 2 * hctb);
-    }
-    u[2] = now();
-    merge_list_a(en, &L);
-    u[3] = now();
-    fprintf(stderr, "[b200] intra DAG: %d tasks in %d levels, widest level %d tasks\n", L.n_task, L.intra_levels, L.intra_width);
-    fprintf(stderr, "[b200] plan (one thread) ms: begin %.3f  PUs %.3f  (-) %.3f  TU validate + intra tasks %.3f | serial tail: PU merge %.3f  intra finish %.3f  list_a merge %.3f\n",
-            1e3 * (t[1] - t[0]), 1e3 * (t[2] - t[1]), 1e3 * (t[3] - t[2]), 1e3 * (t[4] - t[3]), 1e3 * (u[1] - u[0]), 1e3 * (u[2] - u[1]), 1e3 * (u[3] - u[2]));
-  }
-  if (!rc) {
-    merge_list_a(en, &L);
-    plan_finish(&L);
-    counts[0] = (uint32_t)L.n_tiles; counts[1] = (uint32_t)L.n_a; counts[2] = (uint32_t)L.n_aw; counts[3] = (uint32_t)L.n_a8;
-    counts[4] = (uint32_t)L.n_b; counts[5] = (uint32_t)L.n_task; counts[6] = L.ref_mask; counts[7] = 0;
-    auto copy = [](uint32_t* dst, size_t cap_, const std::vector<uint32_t>& v, size_t n) {
-      if (dst) memcpy(dst, v.data(), sizeof(uint32_t) * std::min(cap_, n));
-    };
-    copy(mc_units, cap_units, en->tiles, (size_t)L.n_tiles);
-    copy(list_a, cap_a, en->list_a, (size_t)L.n_a);
-    copy(list_b, cap_b, en->list_b, (size_t)L.n_b);
-    copy(task_start, cap_tasks, en->task_start, L.n_task ? (size_t)L.n_task + 1 : 0);
-  }
-  delete en;
-  return rc;
+  int rc = plan_begin(pl, pic, &L, &cap);
+  if (!rc) rc = plan_build(pl, pic, &L, nullptr);
+  if (rc) return rc;
+  counts[0] = (uint32_t)L.n_tiles; counts[1] = (uint32_t)L.n_a; counts[2] = (uint32_t)L.n_aw; counts[3] = (uint32_t)L.n_a8;
+  counts[4] = (uint32_t)L.n_b; counts[5] = (uint32_t)L.n_task; counts[6] = L.ref_mask; counts[7] = 0;
+  auto copy = [](uint32_t* dst, size_t cap_, const std::vector<uint32_t>& v, size_t n) {
+    if (dst) memcpy(dst, v.data(), sizeof(uint32_t) * std::min(cap_, n));
+  };
+  copy(mc_units, cap_units, pl.tiles, (size_t)L.n_tiles);
+  copy(list_a, cap_a, pl.list_a, (size_t)L.n_a);
+  copy(list_b, cap_b, pl.list_b, (size_t)L.n_b);
+  copy(task_start, cap_tasks, pl.task_start, L.n_task ? (size_t)L.n_task + 1 : 0);
+  return B200_OK;
 }
 
 // Is every access to physical surface `ph` issued on a stream other than `k` complete?  (Same-stream accesses are ordered anyway.)
@@ -1775,7 +1144,7 @@ static int pick_ctx(b200_engine* en, uint32_t ref_mask, int dst_slot)
 // b200_engine_submit_picture spends ~1 ms of host time per 4K picture (validation, work lists, packing), spread over the pool
 // threads but with serial joins; a host that produces pictures faster than that (a parser with several slice / WPP threads, a
 // cache of recorded pictures, bench.py's e2e leg) is held up by it.  The asynchronous path plans WHOLE pictures in parallel: the
-// caller only queues the picture; N planner threads (each with private scratch: a "shadow" engine without CUDA state) validate /
+// caller only queues the picture; N planner threads (each with a Planner of its own: options and scratch) validate /
 // plan / pack one picture each into its staging set; ONE sequencer thread takes the queue in submission order, waits for the
 // picture's plan, and issues the copies and kernels exactly as the synchronous path does — so stream placement, DPB ordering and
 // results are identical.  Reads of finished pictures (b200_engine_read_slot_async) are queued behind the picture they follow.
@@ -1798,9 +1167,9 @@ struct AsyncState {
   std::deque<AsyncCmd*> q;  // submission order; the front is the next one the sequencer executes
   int n_pictures = 0;       // pictures in q (read-backs do not count towards the depth)
   int depth = 12;           // pictures queued at most (B200_ASYNC_QUEUE; <= B200_ASYNC_DEPTH)
-  std::vector<std::thread> planners;
+  std::vector<std::unique_ptr<Planner>> planners;
+  std::vector<std::thread> planner_threads;
   std::thread sequencer;
-  std::vector<b200_engine*> shadows;
   bool stop = false;
   int first_rc = B200_OK;
   std::string first_err;
@@ -1830,7 +1199,7 @@ static int host_cores()
 
 static inline double prof_now() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 
-static void async_planner(b200_engine* en, b200_engine* shadow)
+static void async_planner(b200_engine* en, Planner* pl)
 {
   AsyncState* as = en->async;
   cudaSetDevice(en->device);
@@ -1848,7 +1217,7 @@ static void async_planner(b200_engine* en, b200_engine* shadow)
       cmd->state = 1;
     }
     const double tp0 = en->host_prof ? prof_now() : 0.0;
-    const int rc = plan_and_pack(shadow, &cmd->pic, &cmd->L, *cmd->ss, nullptr);
+    const int rc = plan_and_pack(*pl, &cmd->pic, &cmd->L, *cmd->ss, nullptr);
     const double tp1 = en->host_prof ? prof_now() : 0.0;
     {
       std::lock_guard<std::mutex> lk(as->m);
@@ -1931,23 +1300,21 @@ static int async_start(b200_engine* en)
   try {  // thread creation may throw (resource limits): no exception leaves the C ABI
     as->sequencer = std::thread(async_sequencer, en);
     for (int i = 0; i < n; i++) {
-      b200_engine* sh = new b200_engine();  // no CUDA state: only the planner's scratch and the flags the planner reads
-      sh->device = en->device;
-      sh->region = en->region;
-      sh->mc_legacy = en->mc_legacy;
-      sh->intra_split_planes = en->intra_split_planes;
-      sh->intra_level_order = en->intra_level_order;
-      sh->helper = &en->pool;
-      as->shadows.push_back(sh);
-      as->planners.emplace_back(async_planner, en, sh);
+      as->planners.push_back(std::make_unique<Planner>());
+      Planner& pl = *as->planners.back();
+      pl.opt = en->planner.opt;
+      // a picture with a long plan (a large intra picture) borrows the engine's pool so that the in-order sequencer is not held up by it
+      pl.pool = &en->pool;
+      pl.pool_min_tus = 200000;
+      as->planner_threads.emplace_back(async_planner, en, &pl);
     }
   } catch (const std::exception& ex) {
-    if (as->planners.empty() || !as->sequencer.joinable()) {  // nothing usable: tear down what exists
+    if (as->planner_threads.empty() || !as->sequencer.joinable()) {  // nothing usable: tear down what exists
       async_stop(en);
       return set_err(B200_ERR_NOMEM, "asynchronous submission: cannot start threads (%s)", ex.what());
     }
     // fewer planners than asked for still work
-    as->depth = std::min(as->depth, (int)as->planners.size() + 8);
+    as->depth = std::min(as->depth, (int)as->planner_threads.size() + 8);
   }
   return B200_OK;
 }
@@ -1992,9 +1359,8 @@ static void async_stop(b200_engine* en)
   }
   as->cv_plan.notify_all();
   as->cv_seq.notify_all();
-  for (auto& t : as->planners) t.join();
+  for (auto& t : as->planner_threads) t.join();
   if (as->sequencer.joinable()) as->sequencer.join();
-  for (b200_engine* sh : as->shadows) delete sh;
   delete as;
   en->async = nullptr;
 }
@@ -2063,7 +1429,7 @@ extern "C" int b200_engine_submit_picture(b200_engine* en, const b200_picture* p
   PipeCtx& cx = en->ctx[k];
   StagingSet& ss = en->stage_pool[en->next_stage++ % B200_STAGE_SETS];
   double tp[2] = {0, 0};
-  int rc = plan_and_pack(en, pic, &L, ss, tp);
+  int rc = plan_and_pack(en->planner, pic, &L, ss, tp);
   if (rc) return rc;
   const double t3 = now();
   rc = run_layout(en, k, L, ss.dev, ss.host);
@@ -2086,7 +1452,7 @@ extern "C" int b200_engine_prepare_picture(b200_engine* en, const b200_picture* 
   StagingSet& ss = en->stage_pool[en->next_stage++ % B200_STAGE_SETS];
   b200_picture staged = *pic;
   staged.params.flags &= ~B200_PIC_RECORDS_PINNED;  // a prepared picture keeps its own device copy of everything
-  int rc = plan_and_pack(en, &staged, &pp->L, ss, nullptr);
+  int rc = plan_and_pack(en->planner, &staged, &pp->L, ss, nullptr);
   if (rc) { delete pp; return rc; }
   cudaError_t e = cudaMalloc(&pp->dev, pp->L.total);
   if (e == cudaSuccess) e = cudaMemcpyAsync(pp->dev, ss.host, pp->L.total, cudaMemcpyHostToDevice, cx.stream);

@@ -29,7 +29,8 @@ def plan(lib, pic, region=16):
 
 
 def check_picture(lib, pic, region=16):
-    """`region`: the luma size of an intra region task the planner was run with (B200_REGION)."""
+    """`region`: the luma size of an intra region task the planner was run with (B200_REGION).
+    Returns the number of intra tasks and how many of them merge the planes of a region."""
     r = plan(lib, pic)
     tus, pus = pic.tus, pic.pus
     flags = tus["flags"].astype(int)
@@ -70,7 +71,7 @@ def check_picture(lib, pic, region=16):
     lb, ts = r["lb"], r["ts"]
     assert sorted(lb.tolist()) == np.nonzero(intra)[0].tolist()
     if not len(lb):
-        return 0
+        return 0, 0
     assert ts[0] == 0 and ts[-1] == len(lb) and (np.diff(ts.astype(np.int64)) >= 1).all() and (np.diff(ts.astype(np.int64)) <= 16).all()
     owner = [np.full(((pic.params.height >> (1 if c else 0)) // 4 + 1, (pic.params.width >> (1 if c else 0)) // 4 + 1), -1, np.int64) for c in range(3)]
     task_of = {}
@@ -113,7 +114,7 @@ def check_picture(lib, pic, region=16):
         for (yy, xx) in deps:
             if 0 <= yy < owner[c].shape[0] and 0 <= xx < owner[c].shape[1] and owner[c][yy, xx] >= 0:
                 assert owner[c][yy, xx] <= t, f"TU {i} (task {t}) reads a unit produced by the LATER task {owner[c][yy, xx]}"
-    return len(ts) - 1
+    return len(ts) - 1, n_merged
 
 
 PLANNER_CASES = [("I", (256, 192), {}), ("I", (200, 136), {}), ("B", (320, 192), {}), ("P", (256, 128), dict(special_frac=0.15)),
@@ -124,28 +125,33 @@ PLANNER_CASES = [("I", (256, 192), {}), ("I", (200, 136), {}), ("B", (320, 192),
 def test_planner_work_lists(b200lib, kind, size, kw):
     refs = {} if kind == "I" else dict(ref_slots=(0, 1) if kind == "B" else (0,))
     pic = synth.make_picture(size[0], size[1], kind, seed=77, dst_slot=2, **refs, **kw)
-    n_tasks = check_picture(b200lib, pic)
+    n_tasks, _ = check_picture(b200lib, pic)
     if kind == "I":
         assert n_tasks > 0
 
 
 @pytest.mark.parametrize("env", [{"B200_REGION": "8"}, {"B200_INTRA_ORDER": "level_i"}, {"B200_INTRA_ORDER": "diag"},
-                                 {"B200_REGION": "8", "B200_INTRA_ORDER": "diag"}], ids=lambda e: "-".join(f"{k[5:].lower()}={v}" for k, v in e.items()))
+                                 {"B200_REGION": "8", "B200_INTRA_ORDER": "diag"}, {"B200_INTRA_SPLIT": "0"},
+                                 {"B200_INTRA_SPLIT": "0", "B200_REGION": "8"}, {"B200_INTRA_SPLIT": "0", "B200_INTRA_ORDER": "diag"}], ids=lambda e: "-".join(f"{k[5:].lower()}={v}" for k, v in e.items()))
 @pytest.mark.parametrize("kind,size,kw", PLANNER_CASES)
 def test_planner_work_lists_other_task_shapes(b200lib, monkeypatch, env, kind, size, kw):
-    """The intra task shapes and ticket orders the engine can be switched to (b200_plan_picture_host reads B200_REGION and
-    B200_INTRA_ORDER like b200_engine_create): 8x8-luma regions, and the per-TU level order and CTB anti-diagonal order next
-    to the default region-level order.  The same membership and topological-order properties must hold."""
+    """The intra task shapes and ticket orders the engine can be switched to (b200_plan_picture_host reads the planner's
+    switches like b200_engine_create): 8x8-luma regions, the planes of a region merged into one task in pictures with inter
+    prediction, and the per-TU level order and CTB anti-diagonal order next to the default region-level order.  The same
+    membership and topological-order properties must hold."""
     for k, v in env.items():
         monkeypatch.setenv(k, v)
     refs = {} if kind == "I" else dict(ref_slots=(0, 1) if kind == "B" else (0,))
     pic = synth.make_picture(size[0], size[1], kind, seed=77, dst_slot=2, **refs, **kw)
-    n_tasks = check_picture(b200lib, pic, region=int(env.get("B200_REGION", 16)))
+    region = int(env.get("B200_REGION", 16))
+    n_tasks, n_merged = check_picture(b200lib, pic, region=region)
     if kind == "I":
         assert n_tasks > 0
+    # the switch took effect: merged tasks in P/B pictures (with 8x8 regions every chroma TU is as large as its region: none)
+    assert (n_merged > 0) == (env.get("B200_INTRA_SPLIT") == "0" and kind != "I" and region == 16)
     if env.get("B200_REGION") == "8" and kind == "I":  # the switch took effect: smaller regions, more tasks than with 16x16 regions
         monkeypatch.delenv("B200_REGION")
-        assert n_tasks > check_picture(b200lib, pic)
+        assert n_tasks > check_picture(b200lib, pic)[0]
 
 
 def test_planner_rejects_malformed_records(b200lib):
@@ -179,7 +185,7 @@ def test_planner_on_the_real_1080p_intra_stream(b200lib):
         r.c, r.params = pic, pic.params
         r.tus = np.ctypeslib.as_array(C.cast(pic.tus, C.POINTER(C.c_uint8)), shape=(pic.n_tu * 24,)).view(synth.TU_DT).copy()
         r.pus = np.zeros(0, synth.PU_DT)
-        tasks.append(check_picture(b200lib, r))
+        tasks.append(check_picture(b200lib, r)[0])
         return 0
 
     dec.attach(sink)
