@@ -208,7 +208,7 @@ typedef struct b200_picture {
   const uint8_t*           bs_map;       /* ceil(W/4)*ceil(H/4); may be NULL if deblocking skipped */
   const int8_t*            qp_map;       /* QP_Y per 8x8 luma block, ceil(W/8)*ceil(H/8) */
   const uint8_t*           nofilt_map;   /* per 8x8: bit0 = (pcm && pcm_loop_filter_disable) || cu_transquant_bypass */
-  const uint8_t*           scaling_factors; /* B200_SCALING_FACTOR_BYTES or NULL */
+  const uint8_t*           scaling_factors; /* B200_SCALING_FACTOR_BYTES or NULL; read only under B200_PIC_SCALING_LIST */
 } b200_picture;
 
 /* scaling_factors layout: ScalingFactor_Size0[6][16], Size1[6][64], Size2[6][256], Size3[6][1024]

@@ -11,7 +11,7 @@
 // instruction performs two MACs and the operand loads halve.
 //
 // Arithmetic follows scale_coefficients (transform.cc:361-642) and fallback-dct.cc exactly as tu_residual
-// (kernels_recon.cuh) does: dequant with the 64-bit intermediate and int16 clip (transform.cc:452-525), first-stage
+// (kernels_recon.cuh) does: dequant with the 64-bit intermediate, its low 32 bits clipped to int16 (transform.cc:452-525), first-stage
 // (sum + 64) >> 7 clipped to int16, second stage (sum + rnd) >> (20 - bd) (DST: clipped to int16 again),
 // transform-skip / bypass / RDPCM / rotation (transform.cc:402-448, 548-596; fallback-dct.cc:81-91,161-225).
 #pragma once
@@ -80,7 +80,7 @@ __device__ __forceinline__ int dequant_level(const Dequant& d, const b200_coeff 
   if (d.bypass) return c.level;
   const long long fact = (long long)((d.scl ? d.scl[c.pos] : 1) * d.ls) << d.qd;
   const long long q = ((long long)c.level * fact + (1ll << (d.bd_shift - 1))) >> d.bd_shift;
-  return (int)max(-32768ll, min(32767ll, q));
+  return clip16((int)(unsigned)q);  // the low 32 bits, clipped: the reference's Clip3(int, int, int) (transform.cc:522-523)
 }
 
 // dst[0..N) = Clip(dst + r) with one vector load and one vector store (N = 4 or 8 samples, naturally aligned)

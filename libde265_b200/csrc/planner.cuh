@@ -127,7 +127,7 @@ static int plan_begin(Planner& pl, const b200_picture* pic, PicLayout* L, size_t
   const int w4 = (p.width + 3) / 4, h4 = (p.height + 3) / 4, w8 = (p.width + 7) / 8, h8 = (p.height + 7) / 8;
   L->params = p;
   L->n_tu = pic->n_tu;
-  L->has_scaling = pic->scaling_factors != nullptr;
+  L->has_scaling = (p.flags & B200_PIC_SCALING_LIST) && pic->scaling_factors;  // the factors are valid only under the picture flag
   L->run_deblock = !(p.flags & B200_PIC_SKIP_DEBLOCK) && pic->bs_map && (p.stop_after_stage == B200_STAGE_ALL || p.stop_after_stage == B200_STAGE_DEBLOCK);
   L->run_sao = (p.flags & B200_PIC_SAO_ENABLED) && !(p.flags & B200_PIC_SKIP_SAO) && p.stop_after_stage == B200_STAGE_ALL;
   L->region = pl.opt.region;

@@ -46,6 +46,60 @@ def _zorder(x, y):
 
 _Z = np.array([[_zorder(x, y) for x in range(16)] for y in range(16)], dtype=np.int64)  # [y4][x4] inside a 64x64 CTB
 
+
+def diag_scan(n):
+    """Up-right diagonal scan of an n x n block (H.265 6.5.3): the (x, y) of scan positions 0 .. n*n - 1."""
+    return [(s - y, y) for s in range(2 * n - 1) for y in range(min(s, n - 1), -1, -1) if s - y < n]
+
+
+# H.265 Table 7-6: default ScalingList[1..3][matrixId][i] in up-right diagonal order (Table 7-5: every 4x4 entry is 16)
+DEFAULT_LIST_INTRA = (16, 16, 16, 16, 16, 16, 16, 16, 16, 16, 17, 16, 17, 16, 17, 18, 17, 18, 18, 17, 18, 21, 19, 20, 21, 20, 19, 21, 24, 22, 22, 24,
+                      24, 22, 22, 24, 25, 25, 27, 30, 27, 25, 25, 29, 31, 35, 35, 31, 29, 36, 41, 44, 41, 36, 47, 54, 54, 47, 65, 70, 65, 88, 88, 115)
+DEFAULT_LIST_INTER = (16, 16, 16, 16, 16, 16, 16, 16, 16, 16, 17, 17, 17, 17, 17, 18, 18, 18, 18, 18, 18, 20, 20, 20, 20, 20, 20, 20, 24, 24, 24, 24,
+                      24, 24, 24, 24, 25, 25, 25, 25, 25, 25, 25, 28, 28, 28, 28, 28, 28, 33, 33, 33, 33, 33, 41, 41, 41, 41, 54, 54, 54, 71, 71, 91)
+SCALING_SIZES = ((4, 0), (8, 6 * 16), (16, 6 * 16 + 6 * 64), (32, 6 * 16 + 6 * 64 + 6 * 256))  # (nT, byte offset of matrix 0)
+
+
+def scaling_factor(lst, n, dc=16):
+    """ScalingFactor of one n x n matrix (H.265 7.4.5) from a 16-entry (n = 4) or 64-entry list in up-right diagonal order:
+    the 8x8 list is replicated over (n / 8) x (n / 8) squares for n = 16 / 32, whose position 0 then takes the DC value.
+    Flat at x + n * y, the layout of b200_picture.scaling_factors."""
+    k = 4 if n == 4 else 8
+    m = np.zeros((k, k), np.uint8)
+    for i, (x, y) in enumerate(diag_scan(k)):
+        m[y, x] = lst[i]
+    f = np.kron(m, np.ones((n // k, n // k), np.uint8)).reshape(-1)
+    if n >= 16:
+        f[0] = dc
+    return f
+
+
+def default_scaling_factors():
+    """The spec's default lists (Tables 7-5 / 7-6) expanded with DC 16: matrices 0..2 intra, 3..5 inter at 4x4 to 16x16;
+    32x32 matrix 0 intra, 1 inter (the matrix a 32x32 TU record selects), 2..5 unused in 4:2:0 / 4:0:0 and left flat."""
+    out = np.full(capi.SCALING_FACTOR_BYTES, 16, np.uint8)
+    for n, base in SCALING_SIZES:
+        for m in range(6 if n < 32 else 2):
+            inter = m >= 3 if n < 32 else m == 1
+            out[base + m * n * n:base + (m + 1) * n * n] = scaling_factor((16,) * 16 if n == 4 else DEFAULT_LIST_INTER if inter else DEFAULT_LIST_INTRA, n)
+    return out
+
+
+def max_scaling_factors(rng):
+    """Lists drawn over the whole range the syntax allows (1..255): every matrix holds both 1 and 255, and the DC of every 16x16
+    and 32x32 matrix differs from the entry its 8x8 list puts at position 0."""
+    out = np.zeros(capi.SCALING_FACTOR_BYTES, np.uint8)
+    for n, base in SCALING_SIZES:
+        k = 16 if n == 4 else 64
+        for m in range(6):
+            lst = rng.integers(1, 256, k)
+            lo, hi = rng.choice(k, 2, replace=False)
+            lst[lo], lst[hi] = 1, 255
+            dc = int(rng.integers(1, 255))
+            dc += dc >= lst[0]  # uniform over 1..255 without lst[0]
+            out[base + m * n * n:base + (m + 1) * n * n] = scaling_factor(lst, n, dc)
+    return out
+
 # Reference border of a slot (B200_PAD_X / _Y / _CX / _CY of csrc/dev_common.cuh): MC windows further out are moved to this rim.
 _PAD_X, _PAD_Y, _PAD_CX, _PAD_CY = 128, 80, 64, 40
 
@@ -119,7 +173,9 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
     ``slice_deblock_off_frac`` / ``slice_sao_off_frac``: share of the slices with deblocking off (their edges get bS 0) resp.
     each SAO plane flag off; ``skip_sao``: PIC_SKIP_SAO; ``constrained_intra``: constrained_intra_pred_flag, a neighbour group
     of an intra TU counts as available only if its CU is intra (intrapred.h:557-616, as integration/libde265_hooks.cc records
-    it): only the ``avail`` masks change."""
+    it): only the ``avail`` masks change; ``scaling_list`` True: factors drawn over 1..63 (half of them 16), "default": the
+    spec's default lists (default_scaling_factors), "max": lists over 1..255 (max_scaling_factors) — each sets
+    PIC_SCALING_LIST and marks every coded non-bypass TU with its matrix."""
     assert width % 8 == 0 and height % 8 == 0
     assert chroma_format_idc in (0, 1)
     rng = np.random.default_rng(seed)
@@ -227,7 +283,12 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
             weights[3]["o"][0], weights[3]["o"][1] = [127, -128, 127] * o_scale, [-128, 127, -128] * o_scale
 
     scaling = None
-    if scaling_list:
+    if scaling_list == "default":
+        scaling = default_scaling_factors()
+    elif scaling_list == "max":
+        scaling = max_scaling_factors(rng)
+    elif scaling_list:
+        assert scaling_list is True, scaling_list
         scaling = rng.integers(1, 64, size=capi.SCALING_FACTOR_BYTES).astype(np.uint8)
         scaling[rng.random(capi.SCALING_FACTOR_BYTES) < 0.5] = 16
 

@@ -38,7 +38,9 @@ void orc_dequant(int16_t* coeff_buf, const int16_t* levels, const uint16_t* pos,
   for (int i = 0; i < n; i++) {
     int m = sclist ? sclist[pos[i]] : 1;
     int64_t fact = (int64_t)(m * level_scale[qP % 6]) << (qP / 6);
-    int64_t v = ((int64_t)levels[i] * fact + offset) >> bd_shift;
+    /* transform.cc:522-523 hands the 64-bit value to Clip3(int, int, int) (util.h:89): its low 32 bits are clipped.  Only a
+     * scaling factor above 16 can push the value past the int32 range. */
+    int32_t v = (int32_t)(uint32_t)(((int64_t)levels[i] * fact + offset) >> bd_shift);
     if (v < -32768) v = -32768;
     if (v > 32767) v = 32767;
     coeff_buf[pos[i]] = (int16_t)v;
@@ -828,8 +830,8 @@ static void inter_pred_pu(orc_ctx* c, orc_surface* cur, const b200_picture* pic,
 
 static const uint8_t* scaling_matrix(const b200_picture* pic, const b200_tu* tu)
 {
-  /* transform.cc:489-510 */
-  if (!(tu->flags & B200_TU_SCALING_LIST) || !pic->scaling_factors) return NULL;
+  /* transform.cc:489-510; the factors are valid only under B200_PIC_SCALING_LIST (sps.scaling_list_enable_flag) */
+  if (!(tu->flags & B200_TU_SCALING_LIST) || !(pic->params.flags & B200_PIC_SCALING_LIST) || !pic->scaling_factors) return NULL;
   int nT = 1 << tu->log2_size;
   int m = tu->cidx;
   if (nT == 32) m = 0;
