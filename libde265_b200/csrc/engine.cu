@@ -456,6 +456,17 @@ static int init_tables(int device)
     mc8_build_tables(tb);
     CU(cudaMemcpyToSymbol(c_mc8, &tb, sizeof(tb)));
   }
+  {  // prediction plans of k_intra's small-TU fast path (kernels_recon.cuh)
+    static uint32_t plan[INTRA_PLAN_CLASSES][64];
+    for (int c = 0; c < INTRA_PLAN_CLASSES; c++)
+      for (int lane = 0; lane < 32; lane++) {
+        uint32_t w[2];
+        intra_plan_words(c, lane, w);
+        plan[c][lane] = w[0];
+        plan[c][lane + 32] = w[1];
+      }
+    CU(cudaMemcpyToSymbol(g_intra_plan, plan, sizeof(plan)));
+  }
   if (device < 64) g_tables_ready[device] = true;
   return B200_OK;
 }
