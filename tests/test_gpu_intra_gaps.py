@@ -9,6 +9,7 @@ cases of range_cases.py stage by stage; this file adds the path counts, the intr
 import pytest
 
 import range_cases
+from intra_plan_cases import fast_clamps
 from libde265_b200 import capi, synth
 from libde265_b200.engine import Engine
 from test_gpu_parity import assert_same
@@ -25,15 +26,6 @@ def eng():
     e.close()
 
 
-def clamps(tu):
-    """intra_border_clamps: own column, corner and own row available, each reach available up to a point from its inner end."""
-    q = 1 << (int(tu["log2_size"]) - 2)
-    g, av = (1 << q) - 1, int(tu["avail"])
-    bl, tr = (av >> q) & g, (av >> (capi.AVAIL_TOP_BIT0 + q)) & g
-    own = (av & g) == g and (av >> capi.AVAIL_CORNER_BIT) & 1 and ((av >> capi.AVAIL_TOP_BIT0) & g) == g
-    return bool(own) and not (bl & (bl + 1)) and not (tr & (tr + 1))
-
-
 def path_counts(tus):
     """Per size kind: (general path because of a gap, fast / fused path with only a prefix of a reach available)."""
     gap_classes = {"own_partial", "corner_missing", "reach_gap", "outer_only", "corner_only"}
@@ -41,7 +33,7 @@ def path_counts(tus):
     for tu in tus[(tus["flags"] & capi.TU_INTRA) != 0]:
         log2 = int(tu["log2_size"])
         kind = {2: "4", 3: "8c" if tu["cidx"] else "8y", 4: "16", 5: "32"}[log2]
-        if clamps(tu):
+        if fast_clamps(tu) is not None:
             q = 1 << (log2 - 2)
             full = (1 << q) - 1
             av = int(tu["avail"])
