@@ -7,7 +7,7 @@
 
 #define B200_WARP 32
 
-// Replicated border of every surface plane, in samples (engine.cu surface_ensure; the MC kernels rely on it)
+// Replicated border of every surface plane, in samples (dpb.cuh surface_ensure; the MC kernels rely on it)
 #define B200_PAD_X 128   // luma columns, >= widest MC window - 1
 #define B200_PAD_Y 80    // luma rows
 #define B200_PAD_CX 64   // chroma columns

@@ -11,7 +11,7 @@
 //           luma) and one 3-D TMA box (32 bytes x 14 rows x {Cb, Cr}) per used reference list into shared memory, completion
 //           on an mbarrier.  TMA box origins must be 16-byte aligned in the innermost dimension (measured: an unaligned origin
 //           raises "illegal instruction", tools/tma_probe2.cu), so the box starts at the 16-byte boundary left of the window and
-//           pass 1 picks the window up at its byte offset.  Reference surfaces carry a replicated border (engine.cu), so
+//           pass 1 picks the window up at its byte offset.  Reference surfaces carry a replicated border (dpb.cuh), so
 //           there is no coordinate clamping here: a window further out than the border is moved to the border's rim.
 //           The next batch's boxes are issued as soon as pass 1 has consumed the current windows (they land during pass 2).
 //   pass 1  horizontal filter on bytes, as the reference orders it (fallback-motion.cc:492-560): a task = 2 window rows x 8
@@ -496,7 +496,7 @@ MCT_HD MctBox mct_decode_tile(uint32_t word, int s, const b200_pu* pus, const b2
   const int xf = mvx & 3, yf = mvy & 3, cxf = mvx & 7, cyf = mvy & 7;
   const uint32_t hidx = (xf == 0 && yf == 0) ? 4 : xf;      // full-sample position: gain 64 (<< 6) in pass 1, identity in pass 2
   const uint32_t chidx = (cxf == 0 && cyf == 0) ? 8 : cxf;
-  // window origin = first sample the 8-tap (4-tap) filters touch, moved to the border's rim when further out (see engine.cu)
+  // window origin = first sample the 8-tap (4-tap) filters touch, moved to the border's rim when further out (see dpb.cuh)
   const int wx = mct_clip3(-B200_PAD_X, pic.w + B200_PAD_X - 23, x0 + (mvx >> 2) - 3);
   const int wy = mct_clip3(-B200_PAD_Y, pic.h + B200_PAD_Y - 23, y0 + (mvy >> 2) - 3);
   const int cwx = mct_clip3(-B200_PAD_CX, pic.cw + B200_PAD_CX - 11, (x0 >> 1) + (mvx >> 3) - 1);
