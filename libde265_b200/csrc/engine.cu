@@ -13,12 +13,9 @@
 #include <chrono>
 #include <condition_variable>
 #include <deque>
-#include <exception>
 #include <functional>
 #include <memory>
 #include <mutex>
-#include <string>
-#include <sched.h>
 #include <thread>
 #include <cmath>
 #include <cstdarg>
@@ -130,6 +127,7 @@ struct HostPool {
 };
 
 #include "planner.cuh"
+#include "submit_queue.cuh"
 
 // One pipeline context = one CUDA stream with everything a picture in flight needs privately.  Pictures are issued
 // round-robin onto the contexts; cross-context ordering comes from per-surface events (Dpb, dpb.cuh): a picture waits for
@@ -145,12 +143,12 @@ struct PipeCtx {
   cudaEvent_t tail = nullptr;   // b200_engine_join
 };
 
-struct AsyncState;
 struct b200_engine {
   int device = 0;
   std::atomic<size_t> stage_cap_hint{0};
   std::mutex issue_m;  // held by the asynchronous sequencer while it issues a command (it mutates the Dpb / stream state b200_engine_wait_slot reads)
-  AsyncState* async = nullptr;  // b200_engine_submit_picture_async: planner threads + the in-order sequencer (created on first use)
+  std::unique_ptr<SubmitQueue> async;  // b200_engine_submit_picture_async (created on first use)
+  std::unique_ptr<Planner[]> async_planners;  // one per planner thread of `async`
   PipeCtx ctx[B200_MAX_CTX];
   // Record staging: pinned host buffer + device arena per picture in flight, handed out round-robin whatever stream the picture
   // runs on (a set is reused when the kernels of the picture that used it B200_STAGE_SETS pictures ago have finished)
@@ -182,18 +180,13 @@ struct b200_engine {
   unsigned tcount = 0;           // pictures recorded since enable / reset
   cudaEvent_t* ev = nullptr;     // events of the picture being submitted
   uint64_t launches = 0;
-  double host_s[4] = {0, 0, 0, 0};  // submit_picture host time: [0] validate + staging wait, [1] plan + pack, [3] launches (B200_HOST_PROF=1 prints at destroy)
+  // B200_HOST_PROF=1 prints at destroy: submit_picture's host time (after the first B200_HOST_PROF_SKIP pictures) ...
+  double host_validate = 0, host_plan = 0, host_launch = 0;  // validate + staging wait, plan + pack, launches
   uint64_t host_n = 0;
-  // asynchronous path, same switch: [0] planner busy (sum over threads), [1] sequencer waiting for a plan, [2] sequencer issuing pictures,
-  // [3] sequencer issuing read-backs; run_layout segments: [4] surfaces + H2D copy, [5] order_before, [6] kernels, [7] border + order_after
-  double async_s[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  uint64_t async_n = 0;
-  bool host_prof = false;
-  int host_skip = 0;
+  int host_skip = 0;  // B200_HOST_PROF_SKIP: warm-up pictures left, counted down by both paths (the queue's sequencer while it runs)
+  // ... and run_layout's segments of the pictures the asynchronous queue profiles
+  double seg_surfaces = 0, seg_order_before = 0, seg_kernels = 0, seg_order_after = 0;  // surfaces + H2D copy, order_before, kernels, border + order_after
 };
-
-static int async_flush(b200_engine* en);
-static void async_stop(b200_engine* en);
 
 #define TIMING_RING 256
 
@@ -322,7 +315,6 @@ extern "C" int b200_engine_create(b200_engine** out, int device)
   if (const char* e = getenv("B200_POLL_NS")) en->poll_ns = std::max(32, std::min(100000, atoi(e)));
   if (const char* e = getenv("B200_INTRA_SPIN_LIMIT_MS")) en->spin_limit_ns = 1000000ull * (unsigned long long)std::max(1, std::min(60000, atoi(e)));
   en->tl_path = getenv("B200_TIMELINE");
-  en->host_prof = getenv("B200_HOST_PROF") != nullptr;
   if (const char* e = getenv("B200_HOST_PROF_SKIP")) en->host_skip = std::max(0, atoi(e));
   if (const char* e = getenv("B200_MC_CTAS")) en->mc_ctas = std::max(1, std::min(8, atoi(e)));
   if (const char* e = getenv("B200_STREAMS")) en->n_ctx = std::max(1, std::min(B200_MAX_CTX, atoi(e)));
@@ -353,20 +345,22 @@ extern "C" void b200_engine_destroy(b200_engine* en)
 {
   if (!en) return;
   cudaSetDevice(en->device);
-  async_stop(en);
+  if (en->async) en->async->stop();
   cudaDeviceSynchronize();
   tl_flush(en);
   if (en->tl_base) cudaEventDestroy(en->tl_base);
   dpb_destroy(en->dpb, getenv("B200_HOST_PROF") != nullptr);  // prints the first line of B200_HOST_PROF's report
-  if (getenv("B200_HOST_PROF") && en->async_n)
+  if (getenv("B200_HOST_PROF") && en->async && en->async->prof.pictures) {
+    const SubmitQueue::Prof& a = en->async->prof;
+    const unsigned long long n = a.pictures;
     fprintf(stderr, "[b200] submit_picture_async host ms/picture over %llu pictures: planner busy (all threads) %.3f | sequencer: waiting for a plan %.3f  "
             "pictures %.3f (surfaces+H2D %.3f  order_before %.3f  kernels %.3f  borders+order_after %.3f)  read-backs %.3f\n",
-            (unsigned long long)en->async_n, 1e3 * en->async_s[0] / en->async_n, 1e3 * en->async_s[1] / en->async_n, 1e3 * en->async_s[2] / en->async_n,
-            1e3 * en->async_s[4] / en->async_n, 1e3 * en->async_s[5] / en->async_n, 1e3 * en->async_s[6] / en->async_n, 1e3 * en->async_s[7] / en->async_n,
-            1e3 * en->async_s[3] / en->async_n);
+            n, 1e3 * a.plan_busy / n, 1e3 * a.wait_plan / n, 1e3 * a.issue_pictures / n, 1e3 * en->seg_surfaces / n, 1e3 * en->seg_order_before / n,
+            1e3 * en->seg_kernels / n, 1e3 * en->seg_order_after / n, 1e3 * a.issue_reads / n);
+  }
   if (getenv("B200_HOST_PROF") && en->host_n)
     fprintf(stderr, "[b200] submit_picture host ms/picture over %llu pictures: validate+staging-wait %.3f  plan+pack (threaded) %.3f  launch %.3f\n",
-            (unsigned long long)en->host_n, 1e3 * en->host_s[0] / en->host_n, 1e3 * en->host_s[1] / en->host_n, 1e3 * en->host_s[3] / en->host_n);
+            (unsigned long long)en->host_n, 1e3 * en->host_validate / en->host_n, 1e3 * en->host_plan / en->host_n, 1e3 * en->host_launch / en->host_n);
   for (auto& cx : en->ctx) {
     surface_free(cx.scratch);
     if (cx.sync_buf) cudaFree(cx.sync_buf);
@@ -406,12 +400,20 @@ static int sync_all(b200_engine* en)
   return check_intra_err(en);
 }
 
+// The prologue of the entry points that act after everything queued so far (the synchronous paths keep submission order with
+// the queued pictures): select the device and flush the queue.  Returns (and clears) the first error of a queued command.
+static int flush_queue(b200_engine* en) { return en->async ? en->async->wait(SubmitQueue::all) : B200_OK; }
+static int flushed(b200_engine* en)
+{
+  CU(cudaSetDevice(en->device));
+  return flush_queue(en);
+}
+
 extern "C" int b200_engine_set_streams(b200_engine* en, int n)
 {
   if (!en || n < 1 || n > B200_MAX_CTX) return set_err(B200_ERR_INVALID, "stream count must be 1..%d", B200_MAX_CTX);
-  CU(cudaSetDevice(en->device));
-  { const int frc = async_flush(en); if (frc) return frc; }
-  int rc = sync_all(en);
+  int rc = flushed(en);
+  if (!rc) rc = sync_all(en);
   if (rc) return rc;
   en->n_ctx = n;
   en->next_ctx = 0;
@@ -424,8 +426,8 @@ extern "C" int b200_engine_set_streams(b200_engine* en, int n)
 extern "C" int b200_engine_join(b200_engine* en)
 {
   if (!en) return set_err(B200_ERR_INVALID, "null engine");
-  CU(cudaSetDevice(en->device));
-  { const int frc = async_flush(en); if (frc) return frc; }
+  const int rc = flushed(en);
+  if (rc) return rc;
   for (int k = 1; k < B200_MAX_CTX; k++) {
     CU(cudaEventRecord(en->ctx[k].tail, en->ctx[k].stream));
     CU(cudaStreamWaitEvent(en->ctx[0].stream, en->ctx[k].tail, 0));
@@ -732,7 +734,7 @@ static int run_layout(b200_engine* en, int k, const PicLayout& L, uint8_t* dbase
 {
   PipeCtx& cx = en->ctx[k];
   const b200_pic_params& p = L.params;
-  const bool prof = en->host_prof && en->async && en->host_skip <= 0;
+  const bool prof = en->async && en->async->profiling();
   double tseg[5] = {prof ? prof_now() : 0.0, 0, 0, 0, 0};
   const RefTable refs = dpb_refs(en->dpb, p);
   cudaStream_t streams[B200_MAX_CTX];
@@ -790,7 +792,10 @@ static int run_layout(b200_engine* en, int k, const PicLayout& L, uint8_t* dbase
   dst.valid = true;
   if (prof) {
     tseg[4] = prof_now();
-    for (int i = 0; i < 4; i++) en->async_s[4 + i] += tseg[i + 1] - tseg[i];
+    en->seg_surfaces += tseg[1] - tseg[0];
+    en->seg_order_before += tseg[2] - tseg[1];
+    en->seg_kernels += tseg[3] - tseg[2];
+    en->seg_order_after += tseg[4] - tseg[3];
   }
   return B200_OK;
 }
@@ -851,303 +856,117 @@ static int issue_picture(b200_engine* en, const PicLayout& L, uint8_t* dbase, St
   return B200_OK;
 }
 
-// ---- asynchronous submission ------------------------------------------------------------------------------------------------
-// b200_engine_submit_picture spends ~1 ms of host time per 4K picture (validation, work lists, packing), spread over the pool
-// threads but with serial joins; a host that produces pictures faster than that (a parser with several slice / WPP threads, a
-// cache of recorded pictures, bench.py's e2e leg) is held up by it.  The asynchronous path plans WHOLE pictures in parallel: the
-// caller only queues the picture; N planner threads (each with a Planner of its own: options and scratch) validate /
-// plan / pack one picture each into its staging set; ONE sequencer thread takes the queue in submission order, waits for the
-// picture's plan, and issues the copies and kernels exactly as the synchronous path does — so stream placement, DPB ordering and
-// results are identical.  Reads of finished pictures (b200_engine_read_slot_async) are queued behind the picture they follow.
-struct AsyncCmd {
-  int kind = 0;  // 0 picture, 1 read slot
+// ---- asynchronous submission (submit_queue.cuh) -----------------------------------------------------------------------------
+// Staging sets are handed out round-robin in submission order.  A queued picture's planner writes its set before the picture is
+// issued (and the set marked in flight), so the queue must hold fewer pictures than there are sets: then the picture that used
+// the set before has been issued, and ensure_staging waits for its kernels.
+static_assert(B200_ASYNC_DEPTH < B200_STAGE_SETS, "a staging set would be handed out again before its previous picture was issued");
+static StagingSet& next_staging(b200_engine* en) { return en->stage_pool[en->next_stage++ % B200_STAGE_SETS]; }
+
+// A queued picture (its records, layout and staging set) or read-back (where the planes go).
+struct QueuedCmd : SubmitCmd {
   b200_picture pic{};
   PicLayout L;
   StagingSet* ss = nullptr;
-  int rc = B200_OK;
-  std::string err;
-  int state = 0;  // 0 queued, 1 being planned, 2 planned (guarded by AsyncState::m)
-  int slot = 0;
   void* planes[3] = {nullptr, nullptr, nullptr};
   size_t strides[3] = {0, 0, 0};
-  unsigned long long seq = 0;  // ticket: position in submission order (1, 2, ...)
 };
-struct AsyncState {
-  std::mutex m;
-  std::condition_variable cv_plan, cv_seq, cv_space;
-  std::deque<AsyncCmd*> q;  // submission order; the front is the next one the sequencer executes
-  int n_pictures = 0;       // pictures in q (read-backs do not count towards the depth)
-  int depth = 12;           // pictures queued at most (B200_ASYNC_QUEUE; <= B200_ASYNC_DEPTH)
-  std::vector<std::unique_ptr<Planner>> planners;
-  std::vector<std::thread> planner_threads;
-  std::thread sequencer;
-  bool stop = false;
-  int first_rc = B200_OK;
-  std::string first_err;
-  unsigned long long enq_seq = 0, done_seq = 0;          // tickets: queued last / issued last
-  unsigned long long slot_seq[B200_MAX_SLOTS] = {};      // ticket of the last queued command that writes or reads the slot
-};
-#define B200_ASYNC_DEPTH 32  // queued PICTURES; < B200_STAGE_SETS: a staging set is never handed out again before its previous picture was launched
 
 static int read_slot_async_now(b200_engine* en, int slot, void* const planes[3], const size_t strides[3]);
 
-// Cores this process may use: the affinity mask, clamped by the cgroup v2 CPU quota.
-static int host_cores()
-{
-  int n = (int)std::thread::hardware_concurrency();
-  cpu_set_t set;
-  if (sched_getaffinity(0, sizeof(set), &set) == 0) n = CPU_COUNT(&set);
-  if (FILE* f = fopen("/sys/fs/cgroup/cpu.max", "r")) {
-    char quota[32] = "";
-    long period = 0;
-    if (fscanf(f, "%31s %ld", quota, &period) == 2 && strcmp(quota, "max") != 0 && period > 0) n = std::min(n, std::max(1, (int)((atol(quota) + period - 1) / period)));
-    fclose(f);
-  }
-  return std::max(1, n);
-}
-
-static void async_planner(b200_engine* en, Planner* pl)
-{
-  AsyncState* as = en->async;
-  cudaSetDevice(en->device);
-  for (;;) {
-    AsyncCmd* cmd = nullptr;
-    {
-      std::unique_lock<std::mutex> lk(as->m);
-      for (;;) {
-        if (as->stop) return;
-        for (AsyncCmd* c : as->q)
-          if (c->kind == 0 && c->state == 0) { cmd = c; break; }
-        if (cmd) break;
-        as->cv_plan.wait(lk);
-      }
-      cmd->state = 1;
-    }
-    const double tp0 = en->host_prof ? prof_now() : 0.0;
-    const int rc = plan_and_pack(*pl, &cmd->pic, &cmd->L, *cmd->ss, nullptr);
-    const double tp1 = en->host_prof ? prof_now() : 0.0;
-    {
-      std::lock_guard<std::mutex> lk(as->m);
-      if (en->host_skip <= 0) en->async_s[0] += tp1 - tp0;
-      cmd->rc = rc;
-      if (rc) cmd->err = g_err;
-      cmd->state = 2;
-    }
-    as->cv_seq.notify_all();
-  }
-}
-
-static void async_sequencer(b200_engine* en)
-{
-  AsyncState* as = en->async;
-  cudaSetDevice(en->device);
-  for (;;) {
-    AsyncCmd* cmd = nullptr;
-    double ts[3] = {0, 0, 0};
-    {
-      std::unique_lock<std::mutex> lk(as->m);
-      as->cv_seq.wait(lk, [&] { return as->stop || !as->q.empty(); });  // an empty queue is idle time, not waiting for a plan
-      if (as->stop) return;
-      if (en->host_prof) ts[0] = prof_now();
-      as->cv_seq.wait(lk, [&] { return as->stop || (!as->q.empty() && (as->q.front()->kind != 0 || as->q.front()->state == 2)); });
-      if (as->stop) return;
-      cmd = as->q.front();
-    }
-    if (en->host_prof) ts[1] = prof_now();
-    int rc = cmd->rc;
-    {
-      std::lock_guard<std::mutex> issue(en->issue_m);
-      if (cmd->kind == 0) {
-        if (!rc) rc = issue_picture(en, cmd->L, cmd->ss->dev, cmd->ss);
-      } else {
-        rc = read_slot_async_now(en, cmd->slot, cmd->planes, cmd->strides);
-      }
-    }
-    if (en->host_prof && en->host_skip > 0) {
-      if (cmd->kind == 0) en->host_skip--;  // B200_HOST_PROF_SKIP: warm-up pictures (first-use allocations) stay out of the profile
-    } else if (en->host_prof) {
-      ts[2] = prof_now();
-      en->async_s[1] += ts[1] - ts[0];
-      en->async_s[cmd->kind == 0 ? 2 : 3] += ts[2] - ts[1];
-      if (cmd->kind == 0) en->async_n++;
-    }
-    {
-      std::lock_guard<std::mutex> lk(as->m);
-      if (rc && !as->first_rc) { as->first_rc = rc; as->first_err = cmd->err.empty() ? std::string(g_err) : cmd->err; }
-      as->q.pop_front();
-      if (cmd->kind == 0) as->n_pictures--;
-      as->done_seq = cmd->seq;
-    }
-    delete cmd;
-    as->cv_space.notify_all();
-    as->cv_seq.notify_all();
-  }
-}
-
+// Started on first use: an engine that never submits asynchronously starts no threads.  Each planner thread has a Planner of its
+// own (the engine's options, private scratch); the sequencer issues under issue_m exactly as the synchronous path does, so
+// stream placement, DPB ordering and results are the same.
 static int async_start(b200_engine* en)
 {
   if (en->async) return B200_OK;
-  AsyncState* as = new (std::nothrow) AsyncState();
-  if (!as) return set_err(B200_ERR_NOMEM, "out of memory");
-  en->async = as;
-  // one planner takes ~4 ms of one core per 4K picture: the cores this process may use (affinity mask and cgroup quota: exceeding
-  // the quota gets the whole process throttled) minus four for the caller, the sequencer and the CUDA driver's threads, at most 16
-  // (B200_ASYNC_THREADS overrides)
-  int n = std::max(2, std::min(16, host_cores() - 4));
-  if (const char* e = getenv("B200_ASYNC_THREADS")) n = std::max(1, std::min(32, atoi(e)));
-  as->depth = std::min(B200_ASYNC_DEPTH, n + 8);
-  if (const char* e = getenv("B200_ASYNC_QUEUE")) as->depth = std::max(1, std::min(B200_ASYNC_DEPTH, atoi(e)));
-  try {  // thread creation may throw (resource limits): no exception leaves the C ABI
-    as->sequencer = std::thread(async_sequencer, en);
-    for (int i = 0; i < n; i++) {
-      as->planners.push_back(std::make_unique<Planner>());
-      Planner& pl = *as->planners.back();
-      pl.opt = en->planner.opt;
-      // a picture with a long plan (a large intra picture) borrows the engine's pool so that the in-order sequencer is not held up by it
-      pl.pool = &en->pool;
-      pl.pool_min_tus = 200000;
-      as->planner_threads.emplace_back(async_planner, en, &pl);
-    }
-  } catch (const std::exception& ex) {
-    if (as->planner_threads.empty() || !as->sequencer.joinable()) {  // nothing usable: tear down what exists
-      async_stop(en);
-      return set_err(B200_ERR_NOMEM, "asynchronous submission: cannot start threads (%s)", ex.what());
-    }
-    // fewer planners than asked for still work
-    as->depth = std::min(as->depth, (int)as->planner_threads.size() + 8);
+  const int n = SubmitQueue::planner_threads();
+  en->async_planners.reset(new (std::nothrow) Planner[n]);
+  if (!en->async_planners) return set_err(B200_ERR_NOMEM, "out of memory");
+  for (int i = 0; i < n; i++) {
+    en->async_planners[i].opt = en->planner.opt;
+    // a picture with a long plan (a large intra picture) borrows the engine's pool so that the in-order sequencer is not held up by it
+    en->async_planners[i].pool = &en->pool;
+    en->async_planners[i].pool_min_tus = 200000;
   }
-  return B200_OK;
-}
-
-// Blocks until every queued command has been issued to the GPU; returns (and clears) the first error of a queued command.
-static int async_flush(b200_engine* en)
-{
-  AsyncState* as = en->async;
-  if (!as) return B200_OK;
-  std::unique_lock<std::mutex> lk(as->m);
-  as->cv_space.wait(lk, [&] { return as->q.empty(); });
-  const int rc = as->first_rc;
-  if (rc) set_err(rc, "%s", as->first_err.c_str());
-  as->first_rc = B200_OK;
-  as->first_err.clear();
+  en->async.reset(new (std::nothrow) SubmitQueue());
+  if (!en->async) return set_err(B200_ERR_NOMEM, "out of memory");
+  en->async->plan = [en](int w, SubmitCmd& c) {
+    QueuedCmd& q = static_cast<QueuedCmd&>(c);
+    return plan_and_pack(en->async_planners[w], &q.pic, &q.L, *q.ss, nullptr);
+  };
+  en->async->issue = [en](SubmitCmd& c) {
+    QueuedCmd& q = static_cast<QueuedCmd&>(c);
+    std::lock_guard<std::mutex> issue(en->issue_m);
+    return q.kind == CmdKind::picture ? issue_picture(en, q.L, q.ss->dev, q.ss) : read_slot_async_now(en, q.slot, q.planes, q.strides);
+  };
+  en->async->thread_start = [en] { cudaSetDevice(en->device); };
+  en->async->prof_on = getenv("B200_HOST_PROF") != nullptr;
+  en->async->prof_skip = &en->host_skip;
+  const int rc = en->async->start(n);
+  if (rc) en->async.reset();
   return rc;
-}
-
-// Blocks until every command up to `ticket` has been issued (its records are no longer read by the host side).
-static int async_wait_ticket(b200_engine* en, unsigned long long ticket)
-{
-  AsyncState* as = en->async;
-  if (!as) return B200_OK;
-  std::unique_lock<std::mutex> lk(as->m);
-  if (ticket > as->enq_seq) ticket = as->enq_seq;  // a ticket that was never handed out: everything queued so far
-  as->cv_space.wait(lk, [&] { return as->done_seq >= ticket; });
-  const int rc = as->first_rc;
-  if (rc) set_err(rc, "%s", as->first_err.c_str());
-  as->first_rc = B200_OK;
-  as->first_err.clear();
-  return rc;
-}
-
-static void async_stop(b200_engine* en)
-{
-  AsyncState* as = en->async;
-  if (!as) return;
-  async_flush(en);
-  {
-    std::lock_guard<std::mutex> lk(as->m);
-    as->stop = true;
-  }
-  as->cv_plan.notify_all();
-  as->cv_seq.notify_all();
-  for (auto& t : as->planner_threads) t.join();
-  if (as->sequencer.joinable()) as->sequencer.join();
-  delete as;
-  en->async = nullptr;
-}
-
-static int async_enqueue(b200_engine* en, AsyncCmd* cmd)
-{
-  AsyncState* as = en->async;
-  {
-    std::unique_lock<std::mutex> lk(as->m);
-    as->cv_space.wait(lk, [&] { return as->n_pictures < as->depth && as->q.size() < 4 * B200_ASYNC_DEPTH; });
-    as->q.push_back(cmd);
-    if (cmd->kind == 0) as->n_pictures++;
-    cmd->seq = ++as->enq_seq;
-    const int slot = cmd->kind == 0 ? (int)cmd->pic.params.dst_slot : cmd->slot;
-    if (slot >= 0 && slot < B200_MAX_SLOTS) as->slot_seq[slot] = cmd->seq;
-  }
-  if (cmd->kind == 0) as->cv_plan.notify_one();
-  as->cv_seq.notify_all();
-  return B200_OK;
 }
 
 extern "C" int b200_engine_submit_picture_async(b200_engine* en, const b200_picture* pic)
 {
   if (!en || !pic) return set_err(B200_ERR_INVALID, "null argument");
   CU(cudaSetDevice(en->device));
-  int rc = async_start(en);
+  const int rc = async_start(en);
   if (rc) return rc;
-  AsyncCmd* cmd = new (std::nothrow) AsyncCmd();
+  QueuedCmd* cmd = new (std::nothrow) QueuedCmd();
   if (!cmd) return set_err(B200_ERR_NOMEM, "out of memory");
-  cmd->kind = 0;
+  cmd->slot = pic->params.dst_slot;
   cmd->pic = *pic;  // the record ARRAYS must stay valid until b200_engine_flush / _sync returns
-  cmd->ss = &en->stage_pool[en->next_stage++ % B200_STAGE_SETS];
-  return async_enqueue(en, cmd);
+  cmd->ss = &next_staging(en);
+  en->async->enqueue(cmd);
+  return B200_OK;
 }
 
-extern "C" unsigned long long b200_engine_last_ticket(b200_engine* en)
-{
-  if (!en || !en->async) return 0;
-  std::lock_guard<std::mutex> lk(en->async->m);
-  return en->async->enq_seq;
-}
+extern "C" unsigned long long b200_engine_last_ticket(b200_engine* en) { return en && en->async ? en->async->last_ticket() : 0; }
 
 extern "C" int b200_engine_wait_ticket(b200_engine* en, unsigned long long ticket)
 {
   if (!en) return set_err(B200_ERR_INVALID, "null engine");
-  return async_wait_ticket(en, ticket);
+  return en->async ? en->async->wait(ticket) : B200_OK;
 }
 
 extern "C" int b200_engine_flush(b200_engine* en)
 {
   if (!en) return set_err(B200_ERR_INVALID, "null engine");
-  return async_flush(en);
+  return flush_queue(en);
 }
 
 extern "C" int b200_engine_submit_picture(b200_engine* en, const b200_picture* pic)
 {
   if (!en || !pic) return set_err(B200_ERR_INVALID, "null argument");
-  CU(cudaSetDevice(en->device));
-  {
-    const int frc = async_flush(en);  // keep submission order with pictures queued asynchronously
-    if (frc) return frc;
-  }
+  int rc = flushed(en);
+  if (rc) return rc;
   PicLayout L;
-  StagingSet& ss = en->stage_pool[en->next_stage++ % B200_STAGE_SETS];
+  StagingSet& ss = next_staging(en);
   double tp[2] = {0, 0};
-  int rc = plan_and_pack(en->planner, pic, &L, ss, tp);
+  rc = plan_and_pack(en->planner, pic, &L, ss, tp);
   if (rc) return rc;
   const double t3 = prof_now();
   rc = issue_picture(en, L, ss.dev, &ss);
   if (rc) return rc;
   if (en->host_skip > 0) en->host_skip--;  // B200_HOST_PROF_SKIP: leave the warm-up (first-use allocations) out of the profile
-  else { en->host_s[0] += tp[0]; en->host_s[1] += tp[1]; en->host_s[3] += prof_now() - t3; en->host_n++; }
+  else { en->host_validate += tp[0]; en->host_plan += tp[1]; en->host_launch += prof_now() - t3; en->host_n++; }
   return B200_OK;
 }
 
 extern "C" int b200_engine_prepare_picture(b200_engine* en, const b200_picture* pic, b200_prepared** out)
 {
   if (!en || !pic || !out) return set_err(B200_ERR_INVALID, "null argument");
-  CU(cudaSetDevice(en->device));
-  { const int frc = async_flush(en); if (frc) return frc; }
+  int rc = flushed(en);
+  if (rc) return rc;
   b200_prepared* pp = new (std::nothrow) b200_prepared();
   if (!pp) return set_err(B200_ERR_NOMEM, "out of memory");
   PipeCtx& cx = en->ctx[0];
-  StagingSet& ss = en->stage_pool[en->next_stage++ % B200_STAGE_SETS];
+  StagingSet& ss = next_staging(en);
   b200_picture staged = *pic;
   staged.params.flags &= ~B200_PIC_RECORDS_PINNED;  // a prepared picture keeps its own device copy of everything
-  int rc = plan_and_pack(en->planner, &staged, &pp->L, ss, nullptr);
+  rc = plan_and_pack(en->planner, &staged, &pp->L, ss, nullptr);
   if (rc) { delete pp; return rc; }
   cudaError_t e = cudaMalloc(&pp->dev, pp->L.total);
   if (e == cudaSuccess) e = cudaMemcpyAsync(pp->dev, ss.host, pp->L.total, cudaMemcpyHostToDevice, cx.stream);
@@ -1164,16 +983,15 @@ extern "C" int b200_engine_prepare_picture(b200_engine* en, const b200_picture* 
 extern "C" int b200_engine_run_prepared(b200_engine* en, b200_prepared* pp)
 {
   if (!en || !pp) return set_err(B200_ERR_INVALID, "null argument");
-  CU(cudaSetDevice(en->device));
-  { const int frc = async_flush(en); if (frc) return frc; }
-  return issue_picture(en, pp->L, pp->dev, nullptr);
+  const int rc = flushed(en);
+  return rc ? rc : issue_picture(en, pp->L, pp->dev, nullptr);
 }
 
 extern "C" void b200_engine_free_prepared(b200_engine* en, b200_prepared* pp)
 {
   if (!en || !pp) return;
   cudaSetDevice(en->device);
-  async_flush(en);
+  flush_queue(en);
   sync_all(en);
   if (pp->dev) cudaFree(pp->dev);
   delete pp;
@@ -1182,9 +1000,8 @@ extern "C" void b200_engine_free_prepared(b200_engine* en, b200_prepared* pp)
 extern "C" int b200_engine_sync(b200_engine* en)
 {
   if (!en) return set_err(B200_ERR_INVALID, "null engine");
-  CU(cudaSetDevice(en->device));
-  { const int frc = async_flush(en); if (frc) return frc; }
-  return sync_all(en);
+  const int rc = flushed(en);
+  return rc ? rc : sync_all(en);
 }
 
 template <typename P>
@@ -1201,9 +1018,8 @@ static int utility_write_begin(b200_engine* en, int slot, const b200_pic_params*
   if (!en || !p || slot < 0 || slot >= B200_MAX_SLOTS) return set_err(B200_ERR_INVALID, "bad argument");
   int rc = check_params(*p);
   if (rc) return rc;
-  CU(cudaSetDevice(en->device));
-  { const int frc = async_flush(en); if (frc) return frc; }
-  rc = sync_all(en);
+  rc = flushed(en);
+  if (!rc) rc = sync_all(en);
   if (rc) return rc;
   *s = dpb_acquire(en->dpb, slot, 0, *p, false);  // everything is idle after sync_all: the name keeps its surface, or gets its first one
   if (!*s) return set_err(B200_ERR_NOMEM, "no free picture surface");
@@ -1258,12 +1074,13 @@ extern "C" int b200_engine_read_slot_async(b200_engine* en, int slot, void* cons
 {
   if (!en || !planes || !strides || slot < 0 || slot >= B200_MAX_SLOTS) return set_err(B200_ERR_INVALID, "bad argument");
   if (en->async) {  // pictures are queued: the read takes its place behind them (the picture it reads may not be launched yet)
-    AsyncCmd* cmd = new (std::nothrow) AsyncCmd();
+    QueuedCmd* cmd = new (std::nothrow) QueuedCmd();
     if (!cmd) return set_err(B200_ERR_NOMEM, "out of memory");
-    cmd->kind = 1;
+    cmd->kind = CmdKind::read;
     cmd->slot = slot;
     for (int c = 0; c < 3; c++) { cmd->planes[c] = planes[c]; cmd->strides[c] = strides[c]; }
-    return async_enqueue(en, cmd);
+    en->async->enqueue(cmd);
+    return B200_OK;
   }
   return read_slot_async_now(en, slot, planes, strides);
 }
@@ -1287,8 +1104,7 @@ static int read_slot_async_now(b200_engine* en, int slot, void* const planes[3],
 extern "C" int b200_engine_read_slot(b200_engine* en, int slot, void* const planes[3], const size_t strides[3])
 {
   int rc = b200_engine_read_slot_async(en, slot, planes, strides);
-  if (rc) return rc;
-  rc = async_flush(en);
+  if (!rc) rc = flushed(en);
   if (rc) return rc;
   CU(cudaStreamSynchronize(en->ctx[dpb_read_stream(en->dpb, slot)].stream));
   return check_intra_err(en);
@@ -1299,13 +1115,8 @@ extern "C" int b200_engine_wait_slot(b200_engine* en, int slot)
   if (!en || slot < 0 || slot >= B200_MAX_SLOTS) return set_err(B200_ERR_INVALID, "bad argument");
   CU(cudaSetDevice(en->device));
   if (en->async) {  // not a flush: only the commands that touch this slot (later pictures may still be with the planners)
-    unsigned long long t;
-    {
-      std::lock_guard<std::mutex> lk(en->async->m);
-      t = en->async->slot_seq[slot];
-    }
-    const int frc = async_wait_ticket(en, t);
-    if (frc) return frc;
+    const int rc = en->async->wait(en->async->slot_ticket(slot));
+    if (rc) return rc;
   }
   std::vector<cudaEvent_t> evs;
   {
