@@ -270,7 +270,7 @@ B200_API int  b200_engine_read_slot(b200_engine*, int slot, void* const planes[3
 B200_API int  b200_engine_read_slot_async(b200_engine*, int slot, void* const planes[3], const size_t strides[3]);
 B200_API int  b200_engine_sync(b200_engine*);
 /* Blocks until everything issued so far that writes or reads `slot` has finished (the picture in it is complete and every
- * b200_engine_read_slot_async of it has landed), without waiting for later pictures in other slots: what a decoder calls when it
+ * b200_engine_read_slot_async and b200_engine_export_slot of it has landed), without waiting for later pictures in other slots: what a decoder calls when it
  * hands a picture to the application (push_picture_to_output_queue / de265_get_next_picture, decctx.cc:1842-1881). */
 B200_API int  b200_engine_wait_slot(b200_engine*, int slot);
 /* Page-locked host memory for picture planes that b200_engine_read_slot_async fills without staging (the reference-side binding
@@ -278,8 +278,35 @@ B200_API int  b200_engine_wait_slot(b200_engine*, int slot);
 B200_API void* b200_host_alloc(size_t bytes);
 B200_API void  b200_host_free(void* p);
 
-/* Device pointers of a slot (zero-copy consumers, bench). */
+/* Device pointers of a slot (zero-copy consumers, bench).
+ * Unordered: nothing waits for the picture that writes the slot, and later pictures may overwrite or move the surface while the
+ * caller reads it; use b200_engine_export_slot for an ordered copy. */
 B200_API int  b200_engine_slot_device_planes(b200_engine*, int slot, void* planes[3], size_t strides[3]);
+
+/* Export of a decoded picture into caller-owned CUDA memory (b200_engine_export_slot). */
+#define B200_EXPORT_YUV         0  /* planar Y, Cb, Cr in the picture's own sample type (1 byte <= 8 bit, 2 bytes LE above) */
+#define B200_EXPORT_RGB_BT601   1  /* planar R, G, B, 8 bit */
+#define B200_EXPORT_RGB_BT709   2
+#define B200_EXPORT_RGB_BT2020  3  /* non-constant luminance */
+#define B200_EXPORT_FULL_RANGE  0x01  /* b200_export.flags: full-range input (default: limited / "video" range); RGB only, YUV ignores it */
+
+typedef struct b200_export {
+  uint16_t x, y, width, height;  /* crop window in luma samples; 4:2:0: all four even */
+  uint8_t  format;               /* B200_EXPORT_* */
+  uint8_t  flags;
+  uint8_t  reserved[2];          /* must be 0 */
+} b200_export;                   /* 12 bytes */
+
+/* Enqueue on `stream` (a cudaStream_t on the engine's device; NULL = the legacy default stream) a copy of the crop window of
+ * the picture named `slot` into caller-owned device memory: dst[c] / dst_pitch[c] (bytes) per output plane (YUV: Y, Cb, Cr;
+ * only Y for 4:0:0; RGB: R, G, B).  Returns once the work is enqueued.  Work the caller enqueues on `stream` afterwards sees
+ * the exported picture, and later pictures, fill_slot or upload_slot that write the surface wait for the export.
+ * RGB: nearest chroma (pixel (x, y) takes chroma sample (x >> 1, y >> 1)), integer arithmetic (libde265_b200/csrc/export.cuh).
+ * With b200_engine_submit_picture_async the call blocks until the slot's picture has been issued to the GPU (not until it is
+ * finished), like b200_engine_wait_slot.  A picture damaged by a given-up intra dependency wait is exported as it is; the error
+ * is reported by the next b200_engine_sync / _wait_slot / _read_slot.  b200_engine_wait_slot and _sync also wait for the
+ * exports of the slot / of every slot.  Invalid arguments return B200_ERR_INVALID and leave the engine usable. */
+B200_API int  b200_engine_export_slot(b200_engine*, int slot, const b200_export*, void* const dst[3], const size_t dst_pitch[3], void* stream);
 
 /* Timing of the last submitted picture in milliseconds per stage (CUDA events on the
  * engine stream): [0] H2D, [1] inter pred, [2] recon, [3] deblock V+H, [4] SAO, [5] total.

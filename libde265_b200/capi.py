@@ -94,6 +94,16 @@ class CtbInfo(C.Structure):
                 ("sao_band_pos", C.c_uint8 * 3), ("sao_offset", (C.c_int8 * 4) * 3), ("pad", C.c_uint8 * 3)]
 
 
+EXPORT_YUV, EXPORT_RGB_BT601, EXPORT_RGB_BT709, EXPORT_RGB_BT2020 = 0, 1, 2, 3
+EXPORT_FULL_RANGE = 0x01
+
+
+class Export(C.Structure):
+    """b200_export: crop window in luma samples, B200_EXPORT_* format, flags."""
+    _fields_ = [("x", C.c_uint16), ("y", C.c_uint16), ("width", C.c_uint16), ("height", C.c_uint16),
+                ("format", C.c_uint8), ("flags", C.c_uint8), ("reserved", C.c_uint8 * 2)]
+
+
 class Picture(C.Structure):
     _fields_ = [
         ("params", PicParams),
@@ -107,6 +117,7 @@ class Picture(C.Structure):
 
 assert C.sizeof(PicParams) == 20 and C.sizeof(PU) == 24 and C.sizeof(WeightEntry) == 28
 assert C.sizeof(TU) == 24 and C.sizeof(Coeff) == 4 and C.sizeof(SliceInfo) == 8 and C.sizeof(CtbInfo) == 24
+assert C.sizeof(Export) == 12
 
 PlaneArray = C.c_void_p * 3
 StrideArray = C.c_size_t * 3
@@ -119,6 +130,7 @@ EXPORTS = [
     "b200_engine_launch_count", "b200_engine_stream", "b200_engine_prepare_picture", "b200_engine_run_prepared",
     "b200_engine_free_prepared", "b200_engine_timing_sum", "b200_engine_set_streams", "b200_engine_join", "b200_plan_picture_host", "b200_last_error",
     "b200_engine_wait_slot", "b200_host_alloc", "b200_host_free", "b200_engine_submit_picture_async", "b200_engine_flush", "b200_engine_last_ticket", "b200_engine_wait_ticket",
+    "b200_engine_export_slot",
     "b200_abi_version",
     "b200_rec_create", "b200_rec_destroy", "b200_rec_begin_picture", "b200_rec_add_slice", "b200_rec_add_weights",
     "b200_rec_add_pu", "b200_rec_add_tu", "b200_rec_set_ctb", "b200_rec_bs_map", "b200_rec_qp_map",
@@ -178,6 +190,7 @@ def load(path=None):
     lib.b200_host_free.argtypes = [vp]
     lib.b200_host_free.restype = None
     lib.b200_engine_slot_device_planes.argtypes = [vp, C.c_int, PlaneArray, StrideArray]
+    lib.b200_engine_export_slot.argtypes = [vp, C.c_int, C.POINTER(Export), PlaneArray, StrideArray, vp]
     lib.b200_engine_enable_timing.argtypes = [vp, C.c_int]
     lib.b200_engine_last_timing.argtypes = [vp, C.POINTER(C.c_float * 6)]
     lib.b200_engine_prepare_picture.argtypes = [vp, C.POINTER(Picture), C.POINTER(vp)]

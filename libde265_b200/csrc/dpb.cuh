@@ -185,11 +185,15 @@ static void launch_extend_borders(const Surface& s, cudaStream_t st)
 #define B200_MAX_PHYS (B200_MAX_SLOTS + 32)  // physical surfaces: every name plus the renamed pictures in flight
 
 // Per surface: an access issued on stream k waits only for those on other streams (same-stream accesses are ordered anyway).
+// Exports (b200_engine_export_slot) read on the caller's streams, which are none of the engine's: one external-read event per
+// surface covers all of them, because each export's stream waits for the previous one before it records the event again.
 struct SlotSync {
   cudaEvent_t written = nullptr;
   int writer = -1;                       // stream of the last writer, -1: none in flight
   cudaEvent_t read[B200_MAX_CTX] = {};   // last read of this surface issued on each stream
   bool read_pending[B200_MAX_CTX] = {};
+  cudaEvent_t ext_read = nullptr;        // last export of this surface, on the caller's stream
+  bool ext_pending = false;
 };
 
 struct Dpb {
@@ -211,6 +215,7 @@ static int dpb_init(Dpb& d)
   if (const char* e = getenv("B200_RENAME")) d.rename = atoi(e) != 0;
   for (auto& ss : d.sync) {
     CU(cudaEventCreateWithFlags(&ss.written, cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&ss.ext_read, cudaEventDisableTiming));
     for (auto& e : ss.read) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   }
   return B200_OK;
@@ -227,6 +232,7 @@ static void dpb_destroy(Dpb& d, bool report)
   for (auto& s : d.surf) surface_free(s);
   for (auto& ss : d.sync) {
     if (ss.written) cudaEventDestroy(ss.written);
+    if (ss.ext_read) cudaEventDestroy(ss.ext_read);
     for (auto& e : ss.read)
       if (e) cudaEventDestroy(e);
   }
@@ -252,6 +258,25 @@ static RefTable dpb_refs(Dpb& d, const b200_pic_params& p)
   return refs;
 }
 
+// Blocks until the exports of surface `ph` have finished (before it is freed or reallocated).
+static int dpb_wait_export(Dpb& d, int ph)
+{
+  SlotSync& ss = d.sync[ph];
+  if (ss.ext_pending) CU(cudaEventSynchronize(ss.ext_read));
+  ss.ext_pending = false;
+  return B200_OK;
+}
+
+// Blocks until every export has finished.
+static int dpb_wait_exports(Dpb& d)
+{
+  for (int ph = 0; ph < B200_MAX_PHYS; ph++) {
+    const int rc = dpb_wait_export(d, ph);
+    if (rc) return rc;
+  }
+  return B200_OK;
+}
+
 // Format change (new SPS): drain `streams`, then drop every surface that carries no name — surfaces of another format cannot
 // be reused as they are, and converting them one rename at a time (free + allocate, each a device-wide synchronisation) was
 // measured to leave the second format at 75 % of its speed for a long time.
@@ -261,19 +286,28 @@ static int dpb_set_format(Dpb& d, const b200_pic_params& p, const cudaStream_t* 
   if (d.issued.w && !(d.issued == f)) {
     for (int c = 0; c < n_streams; c++) CU(cudaStreamSynchronize(streams[c]));
     for (int ph = 0; ph < B200_MAX_PHYS; ph++)
-      if (d.owner[ph] < 0 && d.surf[ph].plane[0] && !(format_of(d.surf[ph]) == f)) surface_free(d.surf[ph]);
+      if (d.owner[ph] < 0 && d.surf[ph].plane[0] && !(format_of(d.surf[ph]) == f)) {
+        const int rc = dpb_wait_export(d, ph);
+        if (rc) return rc;
+        surface_free(d.surf[ph]);
+      }
   }
   d.issued = f;
   return B200_OK;
 }
 
-// Is every access to surface `ph` issued on a stream other than `k` complete?  The completed ones are forgotten on the way.
+// Is every access to surface `ph` issued on a stream other than `k` (exports included) complete?  The completed ones are
+// forgotten on the way.
 static bool dpb_idle(Dpb& d, int ph, int k)
 {
   SlotSync& ss = d.sync[ph];
   if (ss.writer >= 0 && ss.writer != k) {
     if (cudaEventQuery(ss.written) != cudaSuccess) return false;
     ss.writer = -1;
+  }
+  if (ss.ext_pending) {
+    if (cudaEventQuery(ss.ext_read) != cudaSuccess) return false;
+    ss.ext_pending = false;
   }
   for (int c = 0; c < B200_MAX_CTX; c++)
     if (c != k && ss.read_pending[c]) {
@@ -289,7 +323,11 @@ static bool dpb_idle(Dpb& d, int ph, int k)
 static Surface* dpb_acquire(Dpb& d, int name, int k, const b200_pic_params& p, bool overlap)
 {
   const int cur = d.lmap[name];
-  if (cur >= 0 && (!d.rename || !overlap || dpb_idle(d, cur, k))) return &d.surf[cur];
+  if (cur >= 0 && (!d.rename || !overlap || dpb_idle(d, cur, k))) {
+    // the name keeps its surface: one of another format is reallocated in place (surface_ensure), not behind its exports
+    if (!(format_of(d.surf[cur]) == format_of(p))) dpb_wait_export(d, cur);
+    return &d.surf[cur];
+  }
   int best = -1, empty = -1, other = -1;
   for (int ph = 0; ph < B200_MAX_PHYS && best < 0; ph++) {
     if (d.owner[ph] >= 0) continue;
@@ -300,7 +338,10 @@ static Surface* dpb_acquire(Dpb& d, int name, int k, const b200_pic_params& p, b
     else if (other < 0) other = ph;
   }
   if (best < 0) best = empty >= 0 ? empty : other;  // a new surface, or an idle one of another format (surface_ensure reallocates it)
-  if (best < 0) return cur >= 0 ? &d.surf[cur] : nullptr;  // pool exhausted: write in place behind the readers (dpb_order_before waits)
+  if (best < 0) {  // pool exhausted: write in place behind the readers (dpb_order_before waits)
+    if (cur >= 0 && !(format_of(d.surf[cur]) == format_of(p))) dpb_wait_export(d, cur);
+    return cur >= 0 ? &d.surf[cur] : nullptr;
+  }
   if (cur >= 0) {
     d.owner[cur] = -1;
     d.n_renamed++;
@@ -313,7 +354,8 @@ static Surface* dpb_acquire(Dpb& d, int name, int k, const b200_pic_params& p, b
 
 // Before a picture issued on stream `k` (`st`) that writes the name `dst` (dpb_acquire): wait for the writers of its reference
 // surfaces and for every earlier reader / writer of its destination surface that ran on another stream (none when the
-// destination was renamed to an idle surface).
+// destination was renamed to an idle surface), exports included: the destination's name never moves with one stream, while
+// timing is on or with B200_RENAME=0.
 static int dpb_order_before(Dpb& d, int k, cudaStream_t st, uint32_t ref_mask, int dst)
 {
   for (int r = 0; r < B200_MAX_SLOTS; r++) {
@@ -325,6 +367,25 @@ static int dpb_order_before(Dpb& d, int k, cudaStream_t st, uint32_t ref_mask, i
   if (sd.writer >= 0 && sd.writer != k) CU(cudaStreamWaitEvent(st, sd.written, 0));
   for (int c = 0; c < B200_MAX_CTX; c++)
     if (c != k && sd.read_pending[c]) CU(cudaStreamWaitEvent(st, sd.read[c], 0));
+  if (sd.ext_pending) CU(cudaStreamWaitEvent(st, sd.ext_read, 0));
+  return B200_OK;
+}
+
+// An export of the picture named `name` on the caller's stream `st`: dpb_export_before orders it after the picture's writer,
+// dpb_export_after after the earlier exports of the surface (whichever streams they ran on), then records the external read
+// that later writers wait for.
+static int dpb_export_before(Dpb& d, int name, cudaStream_t st)
+{
+  const SlotSync& ss = d.sync[d.lmap[name]];
+  if (ss.writer >= 0) CU(cudaStreamWaitEvent(st, ss.written, 0));
+  return B200_OK;
+}
+static int dpb_export_after(Dpb& d, int name, cudaStream_t st)
+{
+  SlotSync& ss = d.sync[d.lmap[name]];
+  if (ss.ext_pending) CU(cudaStreamWaitEvent(st, ss.ext_read, 0));
+  CU(cudaEventRecord(ss.ext_read, st));
+  ss.ext_pending = true;
   return B200_OK;
 }
 
@@ -337,14 +398,15 @@ static int dpb_mark_read(Dpb& d, int name, int k, cudaStream_t st)
   return B200_OK;
 }
 
-// A write of the picture named `name` issued on stream `k` after every earlier access to its surface (dpb_order_before, or a
-// full synchronise).
+// A write of the picture named `name` issued on stream `k` after every earlier access to its surface, exports included
+// (dpb_order_before, or a full synchronise with dpb_wait_exports).
 static int dpb_mark_written(Dpb& d, int name, int k, cudaStream_t st)
 {
   SlotSync& ss = d.sync[d.lmap[name]];
   CU(cudaEventRecord(ss.written, st));
   ss.writer = k;
   for (auto& rp : ss.read_pending) rp = false;  // later accesses wait for this write instead
+  ss.ext_pending = false;
   return B200_OK;
 }
 
@@ -368,7 +430,8 @@ static int dpb_read_stream(const Dpb& d, int name)
 }
 
 // What the host waits for before it touches the picture named `name`: the write of the surface that carries the name, and the
-// reads pending on it and on surfaces that carried the name before (a read-back requested from them may still be in flight).
+// reads and exports pending on it and on surfaces that carried the name before (a read-back requested from them may still be in
+// flight).
 static void dpb_wait_events(const Dpb& d, int name, std::vector<cudaEvent_t>& evs)
 {
   for (int ph = 0; ph < B200_MAX_PHYS; ph++) {
@@ -377,10 +440,11 @@ static void dpb_wait_events(const Dpb& d, int name, std::vector<cudaEvent_t>& ev
     if (current && d.sync[ph].writer >= 0) evs.push_back(d.sync[ph].written);
     for (int c = 0; c < B200_MAX_CTX; c++)
       if (d.sync[ph].read_pending[c]) evs.push_back(d.sync[ph].read[c]);
+    if (d.sync[ph].ext_pending) evs.push_back(d.sync[ph].ext_read);
   }
 }
 
-// After every stream was synchronised: nothing is in flight.
+// After every stream was synchronised and dpb_wait_exports: nothing is in flight.
 static void dpb_forget_pending(Dpb& d)
 {
   for (auto& ss : d.sync) {

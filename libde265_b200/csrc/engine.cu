@@ -57,6 +57,7 @@ static inline double prof_now() { return std::chrono::duration<double>(std::chro
 
 #define B200_MAX_CTX 12  // pipeline streams (PipeCtx)
 #include "dpb.cuh"
+#include "export.cuh"
 
 // ---- engine --------------------------------------------------------------------------------------
 struct StagingSet {
@@ -395,6 +396,8 @@ static int check_intra_err(b200_engine* en)
 static int sync_all(b200_engine* en)
 {
   for (int k = 0; k < B200_MAX_CTX; k++) CU(cudaStreamSynchronize(en->ctx[k].stream));
+  const int rc = dpb_wait_exports(en->dpb);  // fill_slot / upload_slot write behind sync_all without an event
+  if (rc) return rc;
   tl_flush(en);
   dpb_forget_pending(en->dpb);
   return check_intra_err(en);
@@ -1136,6 +1139,64 @@ extern "C" void* b200_host_alloc(size_t bytes)
 extern "C" void b200_host_free(void* p)
 {
   if (p) cudaFreeHost(p);
+}
+
+// Ordered against the engine through the picture store's external reader (dpb_export_before / _after).
+extern "C" int b200_engine_export_slot(b200_engine* en, int slot, const b200_export* ex, void* const dst[3], const size_t dst_pitch[3], void* stream)
+{
+  if (!en || !ex || !dst || !dst_pitch || slot < 0 || slot >= B200_MAX_SLOTS) return set_err(B200_ERR_INVALID, "bad argument");
+  if (ex->format > B200_EXPORT_RGB_BT2020) return set_err(B200_ERR_INVALID, "unknown export format %d", ex->format);
+  if (ex->flags & ~B200_EXPORT_FULL_RANGE) return set_err(B200_ERR_INVALID, "unknown export flags 0x%x", ex->flags);
+  if (ex->reserved[0] || ex->reserved[1]) return set_err(B200_ERR_INVALID, "reserved export bytes must be 0");
+  CU(cudaSetDevice(en->device));
+  if (en->async) {  // the slot's picture may still be queued: wait until it has been issued (not until it is finished)
+    const int rc = en->async->wait(en->async->slot_ticket(slot));
+    if (rc) return rc;
+  }
+  std::lock_guard<std::mutex> issue(en->issue_m);  // the sequencer may be issuing later pictures
+  const Surface* sp = dpb_picture(en->dpb, slot);
+  if (!sp) return set_err(B200_ERR_INVALID, "slot %d holds no picture", slot);
+  const Surface& s = *sp;
+  const int x = ex->x, y = ex->y, w = ex->width, h = ex->height;
+  if (w == 0 || h == 0 || x + w > s.w || y + h > s.h)
+    return set_err(B200_ERR_INVALID, "export window %dx%d at (%d, %d) is empty or outside the %dx%d picture", w, h, x, y, s.w, s.h);
+  if (s.chroma && ((x | y | w | h) & 1)) return set_err(B200_ERR_INVALID, "4:2:0 export window (%d, %d) %dx%d is not even", x, y, w, h);
+  const bool rgb = ex->format != B200_EXPORT_YUV;
+  const int n_out = rgb || s.chroma ? 3 : 1;
+  for (int c = 0; c < n_out; c++) {
+    const size_t row = rgb ? (size_t)w : (size_t)(c ? w / 2 : w) * bytes_per_sample(c ? s.bd_c : s.bd_y);
+    if (!dst[c]) return set_err(B200_ERR_INVALID, "export plane %d missing", c);
+    if (dst_pitch[c] < row) return set_err(B200_ERR_INVALID, "export plane %d: pitch %zu below the row's %zu bytes", c, dst_pitch[c], row);
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc = dpb_export_before(en->dpb, slot, st);
+  if (rc) return rc;
+  const uint8_t* src[3] = {nullptr, nullptr, nullptr};
+  for (int c = 0; c < (s.chroma ? 3 : 1); c++) {
+    const int cx = c ? x / 2 : x, cy = c ? y / 2 : y;
+    src[c] = s.plane[c] + (size_t)cy * s.pitch[c] + (size_t)cx * bytes_per_sample(c ? s.bd_c : s.bd_y);
+  }
+  if (!rgb) {
+    for (int c = 0; c < n_out; c++) {
+      const int bps = bytes_per_sample(c ? s.bd_c : s.bd_y);
+      CU(cudaMemcpy2DAsync(dst[c], dst_pitch[c], src[c], s.pitch[c], (size_t)(c ? w / 2 : w) * bps, c ? h / 2 : h, cudaMemcpyDeviceToDevice, st));
+    }
+  } else {
+    ExportArgs a;
+    for (int c = 0; c < 3; c++) {
+      a.src[c] = src[c];
+      a.src_pitch[c] = s.pitch[c];
+      a.dst[c] = (uint8_t*)dst[c];
+      a.dst_pitch[c] = dst_pitch[c];
+    }
+    a.w = w;
+    a.h = h;
+    a.c = export_coefs(ex->format, (ex->flags & B200_EXPORT_FULL_RANGE) != 0, s.bd_y, s.chroma ? s.bd_c : 8);
+    launch_export_rgb(a, bytes_per_sample(s.bd_y), bytes_per_sample(s.bd_c), !s.chroma, st);
+    en->launches++;
+    CU(cudaGetLastError());
+  }
+  return dpb_export_after(en->dpb, slot, st);
 }
 
 extern "C" int b200_engine_slot_device_planes(b200_engine* en, int slot, void* planes[3], size_t strides[3])

@@ -9,6 +9,7 @@ from . import capi
 class Engine:
     def __init__(self, device=0):
         self.lib = capi.load()
+        self.device = device
         self._h = C.c_void_p()
         capi.check(self.lib.b200_engine_create(C.byref(self._h), device), "b200_engine_create")
 
@@ -64,6 +65,46 @@ class Engine:
         strides = [o.strides[0] for o in out] + [0] * (3 - len(out))
         capi.check(self.lib.b200_engine_read_slot(self._h, slot, capi.PlaneArray(*ptrs), capi.StrideArray(*strides)), "b200_engine_read_slot")
         return out
+
+    _RGB = {"bt601": capi.EXPORT_RGB_BT601, "bt709": capi.EXPORT_RGB_BT709, "bt2020": capi.EXPORT_RGB_BT2020}
+
+    def export(self, slot, params, crop=None, rgb=None, full_range=False, stream=None):
+        """The picture in `slot` as CUDA tensors on the engine's device, enqueued on `stream` (a torch.cuda.Stream; default: the
+        device's current stream), which also allocates the outputs.  Work enqueued on `stream` afterwards sees the picture, and
+        pictures or fill_slot / upload_slot that later write the slot wait for the copy.  ``params`` gives the picture's format (as
+        for read_slot); ``crop`` = (x, y, width, height) in luma samples, even for 4:2:0 (default: the whole picture).
+        Returns [Y, Cb, Cr] (uint8 up to 8 bit, uint16 above; [Y] for 4:0:0), or with ``rgb`` = "bt601" / "bt709" / "bt2020"
+        one (3, height, width) uint8 tensor of planar R, G, B (``full_range``: the samples use the full range, not video range).
+        With submit_async the call blocks until the slot's picture has been issued to the GPU."""
+        import torch
+        if rgb is not None and rgb not in self._RGB:
+            raise ValueError(f"rgb must be one of {sorted(self._RGB)} or None, not {rgb!r}")
+        dev = torch.device("cuda", self.device)
+        if stream is None:
+            stream = torch.cuda.current_stream(dev)
+        x, y, w, h = crop if crop is not None else (0, 0, params.width, params.height)
+        if min(x, y, w, h) < 0 or max(x, y, w, h) > 0xFFFF:
+            raise capi.B200Error(f"export window {crop} outside the 16-bit range of b200_export")
+        with torch.cuda.stream(stream):
+            if rgb is not None:
+                out = torch.empty((3, h, w), dtype=torch.uint8, device=dev)
+                planes = [out[0], out[1], out[2]]
+            else:
+                dt = [torch.uint16 if params.bit_depth_luma > 8 else torch.uint8, torch.uint16 if params.bit_depth_chroma > 8 else torch.uint8]
+                planes = [torch.empty((h, w), dtype=dt[0], device=dev)]
+                if params.chroma_format_idc:
+                    planes += [torch.empty((h // 2, w // 2), dtype=dt[1], device=dev) for _ in range(2)]
+                out = planes
+        ex = capi.Export(x, y, w, h, self._RGB[rgb] if rgb is not None else capi.EXPORT_YUV, capi.EXPORT_FULL_RANGE if full_range else 0)
+        ptrs = [p.data_ptr() for p in planes] + [None] * (3 - len(planes))
+        pitches = [p.stride(0) * p.element_size() for p in planes] + [0] * (3 - len(planes))
+        capi.check(self.lib.b200_engine_export_slot(self._h, slot, C.byref(ex), capi.PlaneArray(*ptrs), capi.StrideArray(*pitches),
+                                                    C.c_void_p(stream.cuda_stream)), "b200_engine_export_slot")
+        return out
+
+    def wait_slot(self, slot):
+        """Blocks until the picture in `slot` and every read-back and export of it have finished."""
+        capi.check(self.lib.b200_engine_wait_slot(self._h, slot), "b200_engine_wait_slot")
 
     def read_slot_into(self, slot, planes_ptrs, strides):
         capi.check(self.lib.b200_engine_read_slot(self._h, slot, capi.PlaneArray(*planes_ptrs), capi.StrideArray(*strides)), "b200_engine_read_slot")
