@@ -149,7 +149,8 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
                  rdpcm_frac=0.0, rotate_frac=0.0, tskip_max_log2=2, chroma_format_idc=1, bit_depth_chroma=None, chroma_qp_offsets=None,
                  lf_offsets=None, weight_range="narrow", sao_offset="random", extreme_mv_frac=0.0, strong_smoothing=True,
                  intra_smoothing_off=False, no_bfilter_on_bypass=False, pcm_lf_disable=False, slice_deblock_off_frac=0.0,
-                 slice_sao_off_frac=0.0, skip_sao=False, constrained_intra=False):
+                 slice_sao_off_frac=0.0, skip_sao=False, constrained_intra=False, coeff_max=None, mv_step=None,
+                 sao_band_pos=(0, 32)):
     """Generate one picture.  ``size_area`` = fraction of the picture area coded as 64/32/16/8 CUs.
     ``tiles`` = (columns, rows) of uniformly spaced tiles (pps.cc uniform_spacing rule): CTBs are then coded in tile-scan
     order and intra availability stops at tile borders (intrapred.h:488-503); ``lf_across_tiles`` False also removes the
@@ -175,7 +176,13 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
     of an intra TU counts as available only if its CU is intra (intrapred.h:557-616, as integration/libde265_hooks.cc records
     it): only the ``avail`` masks change; ``scaling_list`` True: factors drawn over 1..63 (half of them 16), "default": the
     spec's default lists (default_scaling_factors), "max": lists over 1..255 (max_scaling_factors) — each sets
-    PIC_SCALING_LIST and marks every coded non-bypass TU with its matrix."""
+    PIC_SCALING_LIST and marks every coded non-bypass TU with its matrix.
+
+    Filter-steering knobs (same rule: at the default nothing changes): ``coeff_max`` codes every coded TU as one nonzero DC level in
+    [-coeff_max, coeff_max], so residuals shift whole blocks (a flat step at transform edges) instead of adding texture;
+    ``mv_step``: every MV is a multiple of ``mv_step`` luma samples in each component (-2 .. 2 steps), so a reference with
+    steps on its 8x8 grid keeps them on the picture's 8x8 grid when mv_step is a multiple of 8; ``sao_band_pos`` = [lo, hi) of
+    the SAO band positions (29..31 put two or three of the four bands past band 31, onto bands 0..2)."""
     assert width % 8 == 0 and height % 8 == 0
     assert chroma_format_idc in (0, 1)
     rng = np.random.default_rng(seed)
@@ -308,7 +315,11 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
     n_coeff_total = [0]
 
     def gen_coeffs(nT, qp, special):
-        """Returns (positions, levels) of a TU: mostly sparse low-frequency, sometimes dense / extreme."""
+        """Returns (positions, levels) of a TU: mostly sparse low-frequency, sometimes dense / extreme (one DC level with
+        ``coeff_max``)."""
+        if coeff_max is not None:
+            lv = int(rng.integers(1, coeff_max + 1)) * (1 if rng.random() < 0.5 else -1)
+            return np.zeros(1, np.uint16), np.array([lv], np.int16)
         r = rng.random()
         if r < 0.70:
             n = int(rng.integers(1, max(2, nT)))  # sparse
@@ -437,6 +448,8 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
             tu_block(xbase >> 1, ybase >> 1, 2, 2, intra, cmode, qps[2], bypass, ctb_addr, cur_slice, intra)
 
     def rand_mv():
+        if mv_step is not None:
+            return 4 * mv_step * int(rng.integers(-2, 3)), 4 * mv_step * int(rng.integers(-2, 3))
         r = rng.random()
         if r < far_mv_frac:
             return int(rng.integers(-4 * width, 4 * width)), int(rng.integers(-4 * height, 4 * height))
@@ -626,7 +639,7 @@ def make_picture(width, height, pic_type="B", seed=1, bit_depth=8, dst_slot=0, r
             cl, cc = int(rng.integers(0, 4)), int(rng.integers(0, 4))
             ctbs[i]["sao_type"] = tl | (tc << 2) | (tc << 4)
             ctbs[i]["sao_eo_class"] = cl | (cc << 2) | (cc << 4)
-            ctbs[i]["sao_band_pos"] = rng.integers(0, 32, 3)
+            ctbs[i]["sao_band_pos"] = rng.integers(sao_band_pos[0], sao_band_pos[1], 3)
             if lim == lim_c:
                 off = rng.integers(-lim, lim + 1, (3, 4))
             else:
@@ -659,5 +672,45 @@ def random_planes(width, height, bit_depth, seed, bit_depth_chroma=None, chroma_
         img = np.kron(base, np.ones((8, 8), np.int64))[:h, :w] + rng.integers(-40, 41, (h, w))
         ext = rng.random((h, w)) < 0.02  # sprinkle extremes (0 / max) to exercise the int16 wrap of App. A.1
         img = np.where(ext, rng.integers(0, 2, (h, w)) * maxv, img)
+        planes.append(np.ascontiguousarray(np.clip(img, 0, maxv).astype(dt)))
+    return planes
+
+
+def smooth_planes(width, height, bit_depth, seed, steps, bit_depth_chroma=None, chroma_format_idc=1, spikes=()):
+    """Piecewise-smooth reference picture: a gentle ramp over the whole plane (from below 0 to above the maximum, so both
+    clip levels occur) plus a level per 8x8 block that changes from block to block by one of ``steps`` (8-bit units, scaled
+    by 2^(bd - 8); random sign, drawn towards 0 so the levels stay bounded), and on a quarter of the blocks a small texture.
+    The steps sit on the 8x8 grid where deblocking edges lie; choosing them relative to tc and beta at the case's QP makes
+    the filters' off / strong / weak / cut-off outcomes all occur.  ``spikes``: heights (8-bit units) of single-sample spikes
+    on a quarter of the samples at x % 4 and y % 4 in {1, 2}: the deblocking decisions read lines 0 and 3 of an edge segment
+    only, so a spike on line 1 or 2 is filtered as the calm lines decide, and the strong filter's +-2 tc clamps decide the
+    result (MVs on a 16-sample grid keep the spikes on those lines)."""
+    rng = np.random.default_rng(seed)
+    dt = np.uint16 if bit_depth > 8 else np.uint8
+    steps = np.asarray(steps, np.int64)
+    planes = []
+    for c in range(3 if chroma_format_idc else 1):
+        bd = bit_depth if c == 0 or bit_depth_chroma is None else bit_depth_chroma
+        maxv, sc = (1 << bd) - 1, 1 << (bd - 8)
+        w, h = (width, height) if c == 0 else (width // 2, height // 2)
+        bw, bh = (w + 7) // 8, (h + 7) // 8
+
+        def walk(n):  # block levels along one axis: steps from the set, signs pulled back towards 0
+            lv = np.zeros(n, np.int64)
+            for i in range(1, n):
+                d = int(steps[rng.integers(0, len(steps))]) * sc
+                lv[i] = lv[i - 1] + (-d if (lv[i - 1] > 0) == (rng.random() < 0.75) else d)
+            return lv
+        blocks = walk(bw)[None, :] + walk(bh)[:, None]
+        ang = rng.uniform(0, 2 * np.pi)
+        ys, xs = np.mgrid[0:h, 0:w]
+        t = (xs * np.cos(ang) + ys * np.sin(ang)) / max(1.0, abs(w * np.cos(ang)) + abs(h * np.sin(ang)))
+        t -= t.min()
+        ramp = (-0.1 + 1.2 * t / max(t.max(), 1e-9)) * maxv
+        tex = np.kron(rng.random((bh, bw)) < 0.25, np.ones((8, 8), bool))[:h, :w] * rng.integers(-2 * sc, 2 * sc + 1, (h, w))
+        img = np.rint(ramp).astype(np.int64) + np.kron(blocks, np.ones((8, 8), np.int64))[:h, :w] + tex
+        if len(spikes):
+            at = (rng.random((h, w)) < 0.25) & np.isin(ys % 4, (1, 2)) & np.isin(xs % 4, (1, 2))
+            img += at * rng.choice(np.asarray(spikes, np.int64) * sc, (h, w)) * rng.choice([-1, 1], (h, w))
         planes.append(np.ascontiguousarray(np.clip(img, 0, maxv).astype(dt)))
     return planes
